@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- policy steps/sec of the VIMA policy forward pass on B200 (contract: see the task statement).
+"""bench.py -- policy steps/sec of the VIMA policy forward pass on H100.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload cfg3|cfg2|cfg3x|cfg5]
-                    [--precision f16f8] [--ragged] [--graph]
+                    [--precision f16f8] [--ragged] [--graph] [--dump-outputs DIR]
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
 
 One "step" = one policy step for every episode of the batch, exactly as scripts/example.py chains the policy's
@@ -66,6 +66,8 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-gpu-eager", action="store_true")
     ap.add_argument("--no-incremental", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (raw logits, action indices, next action tokens) as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -137,7 +139,7 @@ class Workload:
     def config(self, world: int) -> dict:
         """Identical for both arms (the driver compares them)."""
         cfg = {"workload": self.describe(), "global_batch": world * self.case.B, "parallelism": f"dp{world}",
-               "l2": "inputs larger than L2: activations and packed weights stream from HBM every step (L2 = 126 MB)"}
+               "l2": "inputs larger than L2: activations and packed weights stream from HBM every step (H100 L2 = 50 MB)"}
         if self.name == "cfg3":
             cfg["prompt_len_note"] = ("Lp=256 is BASELINE.md section 4 row #3 / SURVEY 8(d) #3: the reference VIMAPolicy caps prompts at "
                                       "xattn_n_positions=256 (vima_policy.py:26-38); the 512-token prompt is workload cfg3x")
@@ -238,7 +240,7 @@ def norm_logits(dists) -> torch.Tensor:
 # clocks
 # ------------------------------------------------------------------------------------------------------------
 def sample_clocks(stop_evt, out):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
     q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
     dev = os.environ.get("LOCAL_RANK", "0")
@@ -520,6 +522,25 @@ def gpu_eager_leg(wl: Workload, dev, inputs, prompt_tokens, prompt_masks, our_pr
     return out
 
 
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, dists, modes, nxt):
+    """The arrays a caller of the policy step receives, as float32 (indices as float64).  An array over its share of DUMP_BYTES is
+    replaced by a fixed, seeded sample of its flattened elements (same indices on every run of the same shape)."""
+    import numpy as np
+
+    arrays = {"raw_logits": raw_logits(dists).float().cpu().numpy(), "next_action_token": nxt.float().cpu().numpy()}
+    arrays.update({f"mode_{k}": v.double().cpu().numpy() for k, v in modes.items()})
+    os.makedirs(out_dir, exist_ok=True)
+    cap = DUMP_BYTES // len(arrays)
+    for name, a in arrays.items():
+        if a.nbytes > cap:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, cap // a.itemsize, replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+
+
 def run_ours(args):
     import torch.distributed as dist
 
@@ -596,14 +617,17 @@ def run_ours(args):
         barrier()
         e0 = torch.cuda.Event(enable_timing=True); e1 = torch.cuda.Event(enable_timing=True)
         torch.cuda.nvtx.range_push("timed")
+        last = None
         e0.record()
         for _ in range(args.steps):
-            run_step(new_obs_dev)
+            last = run_step(new_obs_dev)
         e1.record()
         barrier()
         torch.cuda.nvtx.range_pop()
         gt.on = False
         ms_total = e0.elapsed_time(e1)
+        if args.dump_outputs and rank == 0 and last is not None:  # before later runs overwrite the graph's output buffers
+            dump_outputs(args.dump_outputs, *last)
         launches = ctx.launches - launches0
         if use_graph:
             launches = policy_step.kernels_per_replay * args.steps
@@ -720,11 +744,10 @@ def run_ours(args):
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak_tf = peaks.get("bf16_tflops_sustained") or 1400.0  # the GEMMs run inside a long step -> sustained figure
-        peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained (of measured)" if peaks else "B200_PROFILING.md fallback 1.4 PF sustained (of fallback)"
+        peak_tf = peaks.get("bf16_tflops_sustained") or 989.0  # the GEMMs run inside a long step -> sustained figure
+        peak_src = "MEASURED_PEAKS.json bf16_tflops_sustained (of measured)" if peaks else "H100 SXM data sheet, dense BF16 989 TFLOP/s at 700 W"
         step_flops = wl.flops_per_episode_step() * B
-        roof = {"bound": "tensor", "peak": peak_tf, "unit": "TFLOP/s", "kernel": "gemm_tc_kernel (tcgen05)", "peak_source": peak_src,
-                "traffic": None, "traffic_note": "per-launch dram bytes of every kernel of the step: profiles/r2_kernel_metrics_step.txt (ncu)",
+        roof = {"bound": "tensor", "peak": peak_tf, "unit": "TFLOP/s", "kernel": "gemm_tc_kernel (wgmma)", "peak_source": peak_src, "traffic": None,
                 "step_algorithmic_tflop": step_flops / 1e12, "step_tflops": step_flops / (ms_step / 1e3) / 1e12,
                 "step_frac_of_peak": step_flops / (ms_step / 1e3) / 1e12 / peak_tf,
                 "note": ("achieved = sum(2MNK) / sum(t) over every gemm_tc_kernel launch of the timed region (CUDA events on the launching stream); "

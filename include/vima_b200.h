@@ -1,5 +1,5 @@
 /*
- * vima_b200 -- C ABI of the B200 (sm_100a) kernels behind the VIMA policy forward pass.
+ * vima_b200 -- C ABI of the H100 (sm_90a) kernels behind the VIMA policy forward pass.
  *
  * The reference (vimalabs/VIMA) is pure Python/PyTorch and has no FFI of its own (SURVEY.md 8(b)); its
  * operator surface is the `vima.nn` module tree.  Every entry point below replaces the arithmetic of one
@@ -24,8 +24,8 @@
  *     VIMA_E_INVALID, so growing a descriptor never makes an old binding read or write through garbage.
  *     `vima_sizeof_*()` report the library's own sizes (bindings assert equality at load time).
  *   - the calling thread's current CUDA device is saved and restored around every call.
- *   - environment (read ONCE, in vima_create): VIMA_B200_ATTN = tc (default) | mma;  VIMA_B200_ATTN_TAIL = kernel (default) | off;  VIMA_B200_GEMM_MODE = 2cta (default) |
- *     mcast | 1cta;  VIMA_B200_EPI_PREFETCH = 0 (default) | 1.
+ *   - environment (read ONCE, in vima_create): VIMA_B200_ATTN = tc (default) | mma;  VIMA_B200_ATTN_TAIL = kernel (default) | off;
+ *     VIMA_B200_EPI_PREFETCH = 0 (default) | 1.
  */
 #ifndef VIMA_B200_H
 #define VIMA_B200_H
@@ -48,15 +48,15 @@ enum { VIMA_ACT_NONE = 0, VIMA_ACT_RELU = 1, VIMA_ACT_QUICKGELU = 2, VIMA_ACT_GE
 typedef struct vima_ctx vima_ctx;
 
 int vima_abi_version(void);
-/* Creates a context on `device` (cudaSetDevice is applied inside every call). Fails if the device is not sm_100. */
+/* Creates a context on `device` (cudaSetDevice is applied inside every call). Fails if the device is not sm_90. */
 int vima_create(vima_ctx** out, int device);
 void vima_destroy(vima_ctx* ctx);
 const char* vima_last_error(vima_ctx* ctx);
 int vima_sm_count(vima_ctx* ctx);
 /* Kernel-selection options, initialised from the environment in vima_create (see "environment" above) and switchable per context:
  * key "attn" = "tc" | "mma";  "attn_tail" = "kernel" | "off" (the <= 8 query rows past the last full 128-row tile: SIMT tail
- * kernel, or one more tcgen05 tile);
- * "gemm_mode" = "2cta" | "mcast" | "1cta";  "epi_prefetch" = "1" | "0".  Unknown key/value: VIMA_E_INVALID. */
+ * kernel, or one more wgmma tile);
+ * "epi_prefetch" = "1" | "0".  Unknown key/value: VIMA_E_INVALID. */
 int vima_set_option(vima_ctx* ctx, const char* key, const char* value);
 /* sizeof() of the descriptor structs as THIS library was compiled (bindings check their mirror structs against these). */
 int vima_sizeof_gemm_desc(void);
@@ -78,7 +78,7 @@ int vima_pack_weight(vima_ctx*, const float* w, int n, int k, int transposed, in
 int vima_pack_weight_f8(vima_ctx*, const float* w, int n, int k, int transposed, int ldw, void* hi8, void* lo8, int ld8, float scale,
                         void* stream);
 
-/* ---- tcgen05 GEMM: out = epilogue(A[M,K] * B[N,K]^T) ------------------------------------------------------
+/* ---- wgmma GEMM: out = epilogue(A[M,K] * B[N,K]^T) ------------------------------------------------------
  * Replaces every large Linear / Conv1D on the path: components.py:87-88,130-142 (c_attn, c_proj, c_fc, query,
  * key_value, attention_out, linear1/2, gated_layer), vit.py:151-157,203-213 (conv1, in/out_proj, mlp),
  * obj_encoder.py:86-93, prompt_encoder.py T5 q/k/v/o/wi/wo, vima_policy.py:49,97-108.

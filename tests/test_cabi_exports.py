@@ -29,7 +29,7 @@ def test_header_symbols_are_exported():
 
 
 def test_no_cpu_fallback():
-    """The product path refuses to run without an sm_100 device instead of silently falling back."""
+    """The product path refuses to run without an sm_90 device instead of silently falling back."""
     import torch
 
     if torch.cuda.is_available():

@@ -17,7 +17,7 @@ pytestmark = pytest.mark.gpu
 
 @pytest.fixture(scope="module", params=["f16x3", "f16f8"])
 def setup(request):
-    """Both the parity default (f16x3) and the mode bench.py runs (f16f8: e4m3 cross terms, cta_group::2 pairs, ghost tiles)."""
+    """Both the parity default (f16x3) and the mode bench.py runs (f16f8: e4m3 cross terms)."""
     import vima_b200
     from tests.policy_runner import build_policy
 

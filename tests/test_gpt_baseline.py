@@ -65,19 +65,15 @@ def test_gpt_state_dict_contract():
     subprocess.run([sys.executable, "-c", code], cwd=root, check=True, env={**os.environ, "PYTHONPATH": root})
 
 
-@pytest.mark.reference
 def test_gpt_spec_matches_reference():
-    import sys
+    """The hand-written spec equals the unmodified reference's state-dict layout (tests/golden/make_ref_specs.py)."""
+    from tests.util import ref_state_dict_spec
 
-    from oracle.ref_shim import load_reference
-
-    load_reference()
-    cfg = synth.GATO_CFGS["gato_tiny"]
-    sd = sys.modules["vima.policy"].VIMAGPTPolicy(**cfg).state_dict()
-    spec = gpt_state_dict_spec(**cfg)
+    sd = ref_state_dict_spec("VIMAGPTPolicy/gato_tiny")
+    spec = gpt_state_dict_spec(**synth.GATO_CFGS["gato_tiny"])
     assert sorted(sd.keys()) == sorted(spec.keys())
     for k, v in sd.items():
-        assert tuple(v.shape) == tuple(spec[k]), k
+        assert v == tuple(spec[k]), k
 
 
 @pytest.mark.gpu

@@ -36,7 +36,7 @@ def test_cached_steps_match_full_history(case_name, mode, tol):
                 full = pol.forward(obs_token=obs_tok[:t + 1], obs_mask=obs_msk[:t + 1], action_token=None if t == 0 else act_tok[:t],
                                    prompt_token=p_tok, prompt_token_mask=p_msk)[-1:]
                 assert step.shape == (1, B, E)
-                # same GEMM / LayerNorm kernels and per-row arithmetic; the attention of these rows runs on the tcgen05 kernel in the
+                # same GEMM / LayerNorm kernels and per-row arithmetic; the attention of these rows runs on the wgmma kernel in the
                 # cached step and -- when the full history leaves <= 8 rows past its last 128-row tile (t = 3: L = 131) -- on the
                 # fp32 SIMT tail kernel in the re-forward: two roundings of the same product.  f16x3 keeps that at the 1e-6 level;
                 # in f16f8 the e4m3 cross-term views of the following GEMMs re-quantise the difference (measured 1.4e-5)

@@ -70,8 +70,8 @@ def test_gemm_plain(ctx, dtname, split, M, N, K):
 @pytest.mark.parametrize("split", [False, True])
 @pytest.mark.parametrize("M,N,K", [(4736, 2304, 768), (4741, 768, 3072), (20000, 768, 768)])
 def test_gemm_cluster_multicast(ctx, split, M, N, K):
-    """Shapes big enough for the 2-CTA cluster path (B tile TMA-multicast to both CTAs), incl. an odd number of m-blocks
-    (ghost tile in the last pair) and a ragged last block; the single-CTA path (VIMA_B200_NO_MCAST) must give the same bits."""
+    """Shapes with more tiles than SMs (every persistent CTA walks several tiles), incl. an odd number of m-blocks and a ragged
+    last block.  (Named after the 2-CTA multicast launch mode these shapes were first written for.)"""
     dt, tdt = DT["f16"]
     g = torch.Generator(device="cuda").manual_seed(M + N)
     A = torch.randn(M, K, device="cuda", generator=g)
@@ -245,8 +245,8 @@ def ref_attention(q, k, v, scale, causal, key_mask, bias):
 
 @pytest.fixture(params=["mma", "tc", "tc+tail_off"])
 def attn_impl(request, ctx):
-    """Both attention kernels: mma.sync (attention.cu) and tcgen05 (attention_tc.cu; shapes it does not take fall back), the latter
-    with its two treatments of the <= 8 rows past the last full 128-row tile: the SIMT tail kernel (default) or one more tcgen05 tile."""
+    """Both attention kernels: mma.sync (attention.cu) and wgmma (attention_tc.cu; shapes it does not take fall back), the latter
+    with its two treatments of the <= 8 rows past the last full 128-row tile: the SIMT tail kernel (default) or one more wgmma tile."""
     impl, _, tail = request.param.partition("+tail_")
     ctx.set_option("attn", impl)
     ctx.set_option("attn_tail", tail or "kernel")

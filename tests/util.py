@@ -67,3 +67,12 @@ def argmax_safe_mask(logits: np.ndarray, dims, margin: float):
         out.append((s[..., -1] - s[..., -2]) > margin)
         off += n
     return np.stack(out, axis=-1)
+
+
+def ref_state_dict_spec(name):
+    """{key: shape} (in state_dict order) of the unmodified reference policy `name`, minted by tests/golden/make_ref_specs.py."""
+    import gzip
+    import json
+
+    with gzip.open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_state_dict_specs.json.gz"), "rt") as fh:
+        return {k: tuple(s) for k, s in json.load(fh)[name]}

@@ -43,7 +43,7 @@ for split in splits:
             kw["out_hi"] = torch.empty(M, n_out, dtype=torch.int16, device="cuda"); kw["out_lo"] = torch.empty_like(kw["out_hi"]) if split == 1 else None
             if split == 2:
                 kw["out_lo8"] = torch.empty(M, n_out, dtype=torch.uint8, device="cuda"); kw["out_hi8"] = torch.empty_like(kw["out_lo8"])
-        if glu: kw["block_n"] = 256
+        if glu: kw["block_n"] = 128
         ctx.gemm(**kw); torch.cuda.synchronize()
         e0 = torch.cuda.Event(enable_timing=True); e1 = torch.cuda.Event(enable_timing=True)
         e0.record()

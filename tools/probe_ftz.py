@@ -1,4 +1,4 @@
-"""GPU probe: do tcgen05 kind::f16 and mma.sync flush fp16 subnormal inputs?"""
+"""GPU probe: do wgmma f16 and mma.sync flush fp16 subnormal inputs?"""
 import math, sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -14,12 +14,12 @@ print("A as fp16 (subnormal) value:", a_hi.view(torch.float16)[0, 0].item())
 out = torch.empty(M, N, device="cuda")
 ctx.gemm(M=M, N=N, K=K, a_hi=a_hi, a_lo=None, lda=K, b_hi=b_hi, b_lo=None, ldb=K, dtype=0, out_f32=out)
 torch.cuda.synchronize()
-print("tcgen05: sum of 64 subnormal*1 =", out[0, 0].item(), "expected", K * tiny, "->", "subnormals HONOURED" if out[0, 0].item() > 0 else "FLUSHED")
+print("wgmma: sum of 64 subnormal*1 =", out[0, 0].item(), "expected", K * tiny, "->", "subnormals HONOURED" if out[0, 0].item() > 0 else "FLUSHED")
 # B subnormal
 ctx.split(W, a_hi, None, dtype=0); A2 = torch.full((N, K), tiny, device="cuda"); ctx.split(A2, b_hi, None, dtype=0)
 ctx.gemm(M=M, N=N, K=K, a_hi=a_hi, a_lo=None, lda=K, b_hi=b_hi, b_lo=None, ldb=K, dtype=0, out_f32=out)
 torch.cuda.synchronize()
-print("tcgen05 (B subnormal):", out[0, 0].item())
+print("wgmma (B subnormal):", out[0, 0].item())
 # mma.sync through the attention kernel: V subnormal constant -> O should equal it
 B, H, L, D = 1, 1, 64, 32
 q = torch.zeros(L, D, device="cuda"); kv = torch.cat([torch.zeros(L, D, device="cuda"), torch.full((L, D), tiny, device="cuda")], 1)

@@ -1,6 +1,6 @@
 """ctypes binding of libvima_b200.so (the C ABI in include/vima_b200.h).
 
-There is NO fallback: if the library is missing or the device is not sm_100, every op raises.  torch is used
+There is NO fallback: if the library is missing or the device is not sm_90, every op raises.  torch is used
 only to own device memory and streams; tensors cross the boundary as raw pointers.
 """
 from __future__ import annotations
@@ -146,8 +146,8 @@ class Context:
         rc = self.lib.vima_create(C.byref(h), int(device))
         if rc != 0:
             raise RuntimeError(
-                f"vima_create(device={device}) failed with code {rc}: vima_b200 needs an sm_100 (B200) device; "
-                "there is no CPU or non-Blackwell fallback"
+                f"vima_create(device={device}) failed with code {rc}: vima_b200 needs an sm_90 (H100) device; "
+                "there is no CPU or non-Hopper fallback"
             )
         self.h = h
         self.device = int(device)
@@ -173,8 +173,7 @@ class Context:
             raise RuntimeError(f"{what} failed (code {rc}): {msg.decode() if msg else ''}")
 
     def set_option(self, key: str, value: str) -> None:
-        """Kernel selection of this context: attn = tc | mma, attn_tail = kernel | off, gemm_mode = 2cta | mcast | 1cta,
-        epi_prefetch = 1 | 0."""
+        """Kernel selection of this context: attn = tc | mma, attn_tail = kernel | off, epi_prefetch = 1 | 0."""
         self._ck(self.lib.vima_set_option(self.h, key.encode(), str(value).encode()), "set_option")
 
     @property

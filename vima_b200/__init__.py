@@ -1,4 +1,4 @@
-"""vima_b200: the VIMA policy forward pass on B200 (sm_100a) kernels behind the reference's `vima` module surface."""
+"""vima_b200: the VIMA policy forward pass on H100 (sm_90a) kernels behind the reference's `vima` module surface."""
 import os
 
 import torch

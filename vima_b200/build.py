@@ -1,4 +1,4 @@
-"""Builds libvima_b200.so (sm_100a) in-tree with nvcc.  `python -m vima_b200.build [--force] [--verbose]`."""
+"""Builds libvima_b200.so (sm_90a) in-tree with nvcc.  `python -m vima_b200.build [--force] [--verbose]`."""
 from __future__ import annotations
 
 import hashlib
@@ -14,7 +14,7 @@ LIB_PATH = os.path.join(OUT_DIR, "libvima_b200.so")
 SOURCES = ["api.cu", "gemm_tc_f16.cu", "gemm_tc_bf16.cu", "norm.cu", "attention.cu", "attention_tc.cu", "attention_tail.cu", "gemm_simt.cu", "misc.cu", "prepare.cu"]
 HEADERS = ["common.cuh", "kernels.h", "gemm_tc.cuh", "gemm_tc_variants.cuh", os.path.join("..", "..", "include", "vima_b200.h")]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "--expt-relaxed-constexpr",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
 ]
 

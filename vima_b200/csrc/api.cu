@@ -23,9 +23,8 @@ struct vima_ctx {
   // environment, read once in vima_create
   int attn_tc;       // VIMA_B200_ATTN: tc (1, default) | mma (0)
   int attn_tail;     // VIMA_B200_ATTN_TAIL: the <= 8 rows past the last full 128-row tile: 1 = "kernel" (default; SIMT tail kernel),
-                     // 0 = "off" (one more tcgen05 tile)
-  int gemm_mode;     // VIMA_B200_GEMM_MODE: 1cta (0) | mcast (1) | 2cta (2, default)
-  int epi_prefetch;  // VIMA_B200_EPI_PREFETCH: L2 prefetch of the next tile's residual / multiplier rows (default 0: A/B in profiles/r2_summary.md)
+                     // 0 = "off" (one more tensor-core tile)
+  int epi_prefetch;  // VIMA_B200_EPI_PREFETCH: L2 prefetch of the next tile's residual / multiplier rows (default 0)
 };
 
 // Restores the calling thread's CUDA device when an entry point returns (the library switches to the context's device).
@@ -102,10 +101,6 @@ int vima_set_option(vima_ctx* c, const char* key, const char* value) {
   } else if (!strcmp(key, "attn_tail")) {
     if (!strcmp(value, "kernel")) { c->attn_tail = 1; return VIMA_OK; }
     if (!strcmp(value, "off")) { c->attn_tail = 0; return VIMA_OK; }
-  } else if (!strcmp(key, "gemm_mode")) {
-    if (!strcmp(value, "1cta")) { c->gemm_mode = 0; return VIMA_OK; }
-    if (!strcmp(value, "mcast")) { c->gemm_mode = 1; return VIMA_OK; }
-    if (!strcmp(value, "2cta")) { c->gemm_mode = 2; return VIMA_OK; }
   } else if (!strcmp(key, "epi_prefetch")) {
     if (!strcmp(value, "0") || !strcmp(value, "1")) { c->epi_prefetch = value[0] == '1'; return VIMA_OK; }
   }
@@ -119,7 +114,7 @@ int vima_create(vima_ctx** out, int device) {
   if (cudaGetDeviceCount(&n) != cudaSuccess || device < 0 || device >= n) return VIMA_E_CUDA;
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return VIMA_E_CUDA;
-  if (prop.major != 10) return VIMA_E_UNSUPPORTED;  // sm_100a code only; there is no fallback path
+  if (prop.major != 9 || prop.minor != 0) return VIMA_E_UNSUPPORTED;  // sm_90a code only; there is no fallback path
   vima_ctx* c = new vima_ctx();
   memset(c, 0, sizeof(*c));
   c->device = device;
@@ -135,10 +130,9 @@ int vima_create(vima_ctx** out, int device) {
     return VIMA_E_CUDA;
   }
   c->encode_tiled = fn;
-  c->attn_tc = 1; c->attn_tail = 1; c->gemm_mode = 2; c->epi_prefetch = 0;
+  c->attn_tc = 1; c->attn_tail = 1; c->epi_prefetch = 0;
   if (const char* e = getenv("VIMA_B200_ATTN")) vima_set_option(c, "attn", e);  // unknown values keep the default
   if (const char* e = getenv("VIMA_B200_ATTN_TAIL")) vima_set_option(c, "attn_tail", e);
-  if (const char* e = getenv("VIMA_B200_GEMM_MODE")) vima_set_option(c, "gemm_mode", e);
   if (const char* e = getenv("VIMA_B200_EPI_PREFETCH")) vima_set_option(c, "epi_prefetch", e);
   c->err[0] = 0;
   *out = c;
@@ -186,7 +180,7 @@ int vima_split_f8(vima_ctx* c, const float* x, int64_t rows, int cols, int ldx, 
 static int choose_block_n(int N, int glu) {
   const int step = glu ? 64 : 32;
   int best = step, best_pad = 1 << 30;
-  for (int bn = step; bn <= 256; bn += step) {
+  for (int bn = step; bn <= GEMM_MAX_BN; bn += step) {
     const int padded = ((N + bn - 1) / bn) * bn;
     if (padded < best_pad || (padded == best_pad && bn > best)) { best = bn; best_pad = padded; }
   }
@@ -253,7 +247,7 @@ int vima_gemm(vima_ctx* c, const vima_gemm_desc* d_in, void* stream) {
     return fail(c, VIMA_E_INVALID, "gemm: out_lo8/out_hi8 come together, with an fp16 out_hi, ld_o8 %% 4 == 0");
   if (d->lda < d->K || d->ldb < d->K) return fail(c, VIMA_E_INVALID, "gemm: leading dimension smaller than K");
   int bn = d->block_n > 0 ? d->block_n : choose_block_n(d->N, d->glu);
-  if (bn > 256 || (bn % (d->glu ? 64 : 32))) return fail(c, VIMA_E_INVALID, "gemm: bad block_n %d", bn);
+  if (bn > GEMM_MAX_BN || (bn % (d->glu ? 64 : 32))) return fail(c, VIMA_E_INVALID, "gemm: bad block_n %d (multiple of 32, 64 with GLU, <= %d)", bn, GEMM_MAX_BN);
   if (d->glu && (d->N % bn)) return fail(c, VIMA_E_INVALID, "gemm: GLU needs N %% block_n == 0");
   {
     const int n_out = d->glu ? d->N / 2 : d->N;
@@ -280,29 +274,20 @@ int vima_gemm(vima_ctx* c, const vima_gemm_desc* d_in, void* stream) {
   memset(&p, 0, sizeof(p));
   const int split = f8 ? 2 : (d->a_lo != nullptr ? 1 : 0);
   int rc;
-  // 2-CTA clusters with a multicast B tile once there is enough work to keep every SM pair busy; VIMA_B200_NO_MCAST=1 disables
   const int tiles_m_ = (d->M + GEMM_BM - 1) / GEMM_BM, tiles_n_ = (d->N + bn - 1) / bn;
-  // VIMA_B200_GEMM_MODE = 1cta | mcast | 2cta (default 2cta: cta_group::2 pairs, M = 256, each CTA stages half of the B tile)
-  const int mode_pref = c->gemm_mode;
-  const bool pair_ok = (bn % 64) == 0 && ((tiles_m_ + 1) / 2) * tiles_n_ >= c->sm_count / 2 && tiles_m_ >= 2;
-  const int mcast = (pair_ok && mode_pref == 1) ? 1 : 0;
-  const int two_cta = (pair_ok && mode_pref == 2) ? 1 : 0;
-  const int b_box = (mcast || two_cta) ? bn / 2 : bn;
   if ((rc = make_tmap(c, &p.tm_a_hi, d->a_hi, d->dtype, d->M, d->K, d->lda, GEMM_BM))) return rc;
-  if ((rc = make_tmap(c, &p.tm_b_hi, d->b_hi, d->dtype, d->N, d->K, d->ldb, b_box))) return rc;
+  if ((rc = make_tmap(c, &p.tm_b_hi, d->b_hi, d->dtype, d->N, d->K, d->ldb, bn))) return rc;
   if (split == 1) {
     if ((rc = make_tmap(c, &p.tm_a_lo, d->a_lo, d->dtype, d->M, d->K, d->lda, GEMM_BM))) return rc;
-    if ((rc = make_tmap(c, &p.tm_b_lo, d->b_lo, d->dtype, d->N, d->K, d->ldb, b_box))) return rc;
+    if ((rc = make_tmap(c, &p.tm_b_lo, d->b_lo, d->dtype, d->N, d->K, d->ldb, bn))) return rc;
   } else if (split == 2) {
     if ((rc = make_tmap_f8(c, &p.tm_a_lo, d->a_lo8, d->M, d->K, d->lda8, GEMM_BM))) return rc;
     if ((rc = make_tmap_f8(c, &p.tm_a_hi8, d->a_hi8, d->M, d->K, d->lda8, GEMM_BM))) return rc;
-    if ((rc = make_tmap_f8(c, &p.tm_b_hi8, d->b_hi8, d->N, d->K, d->ldb8, b_box))) return rc;
-    if ((rc = make_tmap_f8(c, &p.tm_b_lo, d->b_lo8, d->N, d->K, d->ldb8, b_box))) return rc;
+    if ((rc = make_tmap_f8(c, &p.tm_b_hi8, d->b_hi8, d->N, d->K, d->ldb8, bn))) return rc;
+    if ((rc = make_tmap_f8(c, &p.tm_b_lo, d->b_lo8, d->N, d->K, d->ldb8, bn))) return rc;
   }
   p.M = d->M; p.N = d->N; p.K = d->K;
   p.block_n = bn;
-  p.mcast = mcast;
-  p.two_cta = two_cta;
   p.split = split;
   p.dtype = d->dtype;
   p.glu = d->glu;
@@ -319,16 +304,15 @@ int vima_gemm(vima_ctx* c, const vima_gemm_desc* d_in, void* stream) {
   p.res_stats = d->res_stats; p.res_gamma = d->res_gamma; p.res_beta = d->res_beta;
   p.stats_out = d->stats_out; p.stats_parts = d->stats_parts;
 
-  const size_t stage = (size_t)(GEMM_A_TILE_BYTES + (two_cta ? bn / 2 : bn) * 128) * (split ? 2 : 1);
-  const size_t fixed = gemm_smem_bytes(bn, split, 0, two_cta);
+  const size_t stage = (size_t)(GEMM_A_TILE_BYTES + bn * 128) * (split ? 2 : 1);
+  const size_t fixed = gemm_smem_bytes(bn, split, 0);
   int n_stages = (int)(((size_t)c->max_smem_optin - fixed) / stage);
   if (n_stages > GEMM_MAX_STAGES) n_stages = GEMM_MAX_STAGES;
   if (n_stages < 2) return fail(c, VIMA_E_UNSUPPORTED, "gemm: not enough shared memory for 2 stages");
   p.n_stages = n_stages;
-  const size_t smem = gemm_smem_bytes(bn, split, n_stages, two_cta);
-  const int tiles = mcast ? ((tiles_m_ + 1) / 2) * tiles_n_ : tiles_m_ * tiles_n_;  // work units
-  int grid = tiles < c->sm_count ? tiles : c->sm_count;
-  if (mcast || two_cta) grid = 2 * (tiles < c->sm_count / 2 ? tiles : c->sm_count / 2);
+  const size_t smem = gemm_smem_bytes(bn, split, n_stages);
+  const int tiles = tiles_m_ * tiles_n_;
+  const int grid = tiles < c->sm_count ? tiles : c->sm_count;  // persistent: one CTA per SM walks the tiles
   GemmLaunch l;
   l.act = d->act; l.glu = d->glu != 0; l.mul = d->mul != nullptr; l.res = d->residual != nullptr;
   l.o32 = d->out_f32 != nullptr; l.o16 = d->out_hi != nullptr; l.dtype = d->dtype;
@@ -406,14 +390,11 @@ int vima_attention(vima_ctx* c, const vima_attn_desc* d_in, void* stream) {
     return fail(c, VIMA_E_INVALID, "attention: kv_batch_rows / mask_ld must cover Lk, q_pos0 >= 0");
   if ((p.o_lo8 == nullptr) != (p.o_hi8 == nullptr) || (p.o_lo8 && ((p.ldo8 & 1) || d->dtype != DT_F16)))
     return fail(c, VIMA_E_INVALID, "attention: o_lo8/o_hi8 come together (fp16 format, even ldo8)");
-  // tcgen05 kernel for the shapes it takes (head_dim 32, split operands, no relative bias), mma.sync kernel otherwise;
+  // wgmma kernel for the shapes it takes (head_dim 32, split operands, no relative bias), mma.sync kernel otherwise;
   // VIMA_B200_ATTN=mma (read once in vima_create) forces the latter.  Both are covered by the kernel tests.
   if (c->attn_tc && attention_tc_supported(p)) {
-    // the tcgen05 kernel works on 128-row query tiles: a few rows past the last full tile (7 of 263, 8 of 392) would hold a CTA slot
-    // for the whole key range with one warp of four at work -- they go to the SIMT tail kernel instead (attention_tail.cu).
-    // Measured per decoder layer at the benchmark shape (self + cross, B = 256, L = 263): 1.71 ms with one more tcgen05 tile,
-    // 1.58 ms with the tail kernel; running the same routine inside the CTA of the last full tile was slower than both (1.80 ms:
-    // it extends the lifetime of a CTA that holds TMEM and 76 KB of shared memory) and was dropped (profiles/r2i_*).
+    // the wgmma kernel works on 128-row query tiles: a few rows past the last full tile (7 of 263, 8 of 392) would hold a CTA slot
+    // for the whole key range with one warp of eight at work -- they go to the SIMT tail kernel instead (attention_tail.cu).
     const int tail = p.Lq % 128;
     if (c->attn_tail && p.Lq > 128 && tail >= 1 && tail <= ATTN_TAIL_MAX_ROWS) {
       AttnParams body = p;

@@ -148,7 +148,7 @@ __global__ void __launch_bounds__(256, (D == 32) ? 2 : 1) attention_kernel(const
 #pragma unroll
       for (int nt = 0; nt < 8; ++nt) s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.f;
       // MMAs are issued round-robin over 4 independent accumulators so that back-to-back HMMAs never depend on each
-      // other (a chain of 6 dependent HMMAs per accumulator left the pipe 60 % idle: profiles/r1_summary.md section 3)
+      // other (a chain of 6 dependent HMMAs per accumulator leaves the pipe waiting on each result)
 #pragma unroll
       for (int half = 0; half < 2; ++half) {
 #pragma unroll

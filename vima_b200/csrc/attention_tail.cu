@@ -1,10 +1,9 @@
 // Tail rows of the decoder attentions (head_dim 32), companion of attention_tc.cu.
 //
-// The tcgen05 kernel works on 128-query tiles.  The decoder's sequence lengths are T*(Q+1)-1 (263 for the 200M benchmark
+// The wgmma kernel works on 128-query tiles.  The decoder's sequence lengths are T*(Q+1)-1 (263 for the 200M benchmark
 // configuration, 392 = prompt | sep | history for VIMA-Gato): a handful of rows (7 / 8) spill into one more tile per (batch, head)
-// that occupies a CTA slot for its whole key range while one warp of four has work -- measured at 31 % of the self-attention and
-// 29 % of the cross-attention kernel time (L = 263 vs 256, profiles/r2f).  Those rows are taken here instead: a warp per
-// (batch, head), up to 8 query rows, plain fp32 FMAs (packed f32x2) on the (hi + lo) operands -- about 2 MFLOP per unit, no tensor
+// that occupies a CTA slot for its whole key range while one warp of eight has work.  Those rows are taken here instead: a warp per
+// (batch, head), up to 8 query rows, plain fp32 FMAs on the (hi + lo) operands -- about 2 MFLOP per unit, no tensor
 // cores, no shared-memory staging of K / V (each element is read exactly once, straight from L2).
 //
 //   phase 1  lane = key:    y[j][i] = (q_i * scale*log2e) . k_j  + mask terms      -> shared [Lk][8], running row maxima
@@ -42,17 +41,17 @@ __device__ __forceinline__ float2 unpack64(unsigned long long v) {
   asm("mov.b64 {%0, %1}, %2;" : "=f"(r.x), "=f"(r.y) : "l"(v));
   return r;
 }
-// acc += a * b on two packed fp32 lanes
+// acc += a * b on two packed fp32 lanes (two scalar FFMAs: sm_90 has no packed fp32 FMA)
 __device__ __forceinline__ void ffma2(unsigned long long& acc, unsigned long long a, unsigned long long b) {
-  asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(acc) : "l"(a), "l"(b));
+  const float2 x = unpack64(acc), y = unpack64(a), z = unpack64(b);
+  acc = pack2(fmaf(y.x, z.x, x.x), fmaf(y.y, z.y, x.y));
 }
 
 template <int DT>
 __global__ void __launch_bounds__(TAIL_WARPS * 32) attention_tail_kernel(const AttnParams p, int row0, int nt, int lk_pad) {
   extern __shared__ __align__(16) float smt[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // (batch ascending, like the tcgen05 kernel before it: walking the batch downwards to catch that kernel's last K / V rows in L2
-  //  was measured 45 % SLOWER -- 0.246 vs 0.169 ms per call, profiles/r2l_*)
+  // (batch ascending, like the wgmma kernel before it)
   const long long unit = (long long)blockIdx.x * TAIL_WARPS + warp;
   if (unit >= (long long)p.B * p.H) return;  // whole warps leave; nothing below synchronises across warps
   const int b = (int)(unit / p.H), h = (int)(unit % p.H);

@@ -1,25 +1,20 @@
-// tcgen05 attention for the decoder's hot shapes (head_dim 32, (hi, lo) operand pairs, no relative bias), round-2 design:
+// wgmma attention for the decoder's hot shapes (head_dim 32, (hi, lo) operand pairs, no relative bias):
 //
-//   one CTA per (batch, head, 128-query-row tile); keys stream through in chunks of 64.  Warps 0-3 = softmax (thread = query
-//   row = TMEM lane), warp 4 = control (one lane issues every TMA load and every MMA; the warp owns the TMEM allocation).
-//
-//   control lane, per chunk c:   QK(c+1):  S[128x64] = Q K^T         6 x tcgen05.mma M128 N64 K16 (hi*hi, lo*hi, hi*lo), as soon
-//                                          as the softmax warps have pulled S(c) into registers (s_free) -> S(c+1) is ready when
-//                                          they come back; TMA brings K(c+2) / V(c+1) in behind the MMAs that free their slots
-//                                PV(c):    O[128x32] += P V          12 x tcgen05.mma M128 N32 K16 once P(c) is in shared memory
-//   softmax thread, per chunk:   tcgen05.ld its 64 scores (ONE pass over TMEM: its 64 B/clk read port, MUFU and issue all top
-//                                out near 16 elements/clk/SM), max with FMNMX3, exp2 with the scale folded into a packed FFMA2,
-//                                (hi, lo) fp16 split, 128-bit stores into the 128B-swizzled K-major tile the MMA reads.
-//   O stays in TMEM for the whole key range: the running maximum is only raised when a chunk exceeds it by more than 2^8 (the
-//   row's O / l are then rescaled through tcgen05.ld/st), so P <= 256 fits fp16 and the per-chunk read-modify-write of O, its
-//   barrier round trip and the online-softmax correction of the round-1 kernel are gone.  The softmax warps never wait for an
-//   MMA they did not need: the only waits are "S(c) ready" and "P buffer free".
+//   one CTA per (batch, head, 128-query-row tile), two warpgroups of 64 query rows each; keys stream through in chunks of 64.
+//   per chunk c, every warpgroup:
+//     S[64x64] = Q K^T     6 x wgmma M64 N64 K16 (hi*hi, lo*hi, hi*lo), Q and K(c) from shared memory (TMA, 64-byte swizzle);
+//                          K(c+2) is loaded by TMA into the slot K(c) leaves
+//     V(c) -> V^T          while S is computed, every thread loads 8 values of V(c) (hi and lo) and writes them transposed into
+//                          a 128-byte-swizzled K-major tile, the B operand layout wgmma reads
+//     softmax              in registers on the accumulator fragment (4 lanes share a row), online maximum, exp2 with the scale
+//                          folded into the FMA; P as (hi, lo) 16-bit pairs stays in registers
+//     O[64x32] += P V      12 x wgmma M64 N32 K16 with A = P from registers, B = V^T from shared memory
 //
 // Same mask semantics as attention.cu (reference components.py:51-80): the causal constant is the reference's soft -1e4, key
 // padding adds finfo.min, keys beyond Lk are excluded.  A causal tile first runs the chunks up to its diagonal; hidden keys have
 // weight exp(-1e4 - m) == 0 exactly in fp32 once m > -1e4 + 104, so stopping there is bit-compatible with the reference's
 // full-width softmax.  If some row has only seen padded keys by then (m still <= -9000), the tile is re-run over every chunk
-// with the exact formulas (rare: the first history slot is always valid in VIMA's data).
+// (rare: the first history slot is always valid in VIMA's data).
 #include "kernels.h"
 
 namespace vima {
@@ -30,121 +25,56 @@ constexpr float FP32_MIN_TC = -3.4028234663852886e38f;
 constexpr float LOG2E_TC = 1.4426950408889634f;
 constexpr float CAUSAL_L2_TC = -1e4f * LOG2E_TC;
 constexpr float EXIT_L2_TC = -9000.f * LOG2E_TC;
-constexpr float LAZY_THRESH = 8.0f;  // log2(256): raise the reference maximum only when a chunk beats it by more than this
 
-constexpr int ATC_THREADS = 160;
+constexpr int ATC_THREADS = 256;
 constexpr int ATC_BM = 128, ATC_KC = 64, ATC_D = 32;
-constexpr int ATC_TMEM_COLS = 128;   // S: columns [0, 64), O: [64, 96)
 constexpr int ATC_MAX_LK = 512;      // mask row held in shared memory as floats
 // shared memory carve (bytes; swizzled tiles 1024-aligned)
-constexpr int OFF_QH = 0, OFF_QL = 8192;
-constexpr int OFF_K = 16384;                 // 2 stages x {hi 4096, lo 4096}
-constexpr int OFF_VH = 32768, OFF_VL = 36864;
-constexpr int OFF_PH = 40960, OFF_PL = 57344;
-constexpr int OFF_MASK = 73728;              // float[512]
-constexpr int OFF_FLAG = OFF_MASK + ATC_MAX_LK * 4;  // int[8]: per-chunk "any key masked"
-constexpr int OFF_BAR = OFF_FLAG + 32;       // 8 mbarriers
-constexpr int OFF_TPTR = OFF_BAR + 64;
-constexpr int ATC_SMEM = OFF_TPTR + 16;
+constexpr int OFF_QH = 0, OFF_QL = 8192;     // 128 rows x 64 B each
+constexpr int OFF_K = 16384;                 // 2 stages x {hi 4096, lo 4096}: 64 keys x 64 B
+constexpr int OFF_VT = 32768;                // 2 buffers x {hi 4096, lo 4096}: V^T, 32 dims x 128 B
+constexpr int OFF_MASK = 49152;              // float[512]
+constexpr int OFF_BAR = OFF_MASK + ATC_MAX_LK * 4;  // 3 mbarriers
+constexpr int ATC_SMEM = OFF_BAR + 32;
 
 struct AttnTcParams {
   AttnParams a;
-  CUtensorMap tm_q_hi, tm_q_lo, tm_k_hi, tm_k_lo, tm_v_hi, tm_v_lo;
+  CUtensorMap tm_q_hi, tm_q_lo, tm_k_hi, tm_k_lo;
 };
 
-__device__ __forceinline__ uint64_t desc_sw64(uint32_t a) {
-  return (uint64_t)((a >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)(512 >> 4) << 32) | (1ull << 46) | (4ull << 61);
-}
-__device__ __forceinline__ uint64_t desc_sw128(uint32_t a) {
-  return (uint64_t)((a >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-
-__device__ __forceinline__ float max3(float a, float b, float c) {
-  float r;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
+__device__ __forceinline__ unsigned short e4m3x2(float x0, float x1) {  // low byte = x0
+  unsigned short r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(x1), "f"(x0));
   return r;
 }
-// (x0, x1) * s + n  as one packed FFMA2
-__device__ __forceinline__ void fma2(float& x0, float& x1, float s, float n) {
-  unsigned long long xx, ss, nn;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(xx) : "f"(x0), "f"(x1));
-  asm("mov.b64 %0, {%1, %1};" : "=l"(ss) : "f"(s));
-  asm("mov.b64 %0, {%1, %1};" : "=l"(nn) : "f"(n));
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(xx) : "l"(xx), "l"(ss), "l"(nn));
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(x0), "=f"(x1) : "l"(xx));
-}
 
-// (x0, x1) * s + (n0, n1)  as one packed FFMA2
-__device__ __forceinline__ void fma2v(float& x0, float& x1, float s, float n0, float n1) {
-  unsigned long long xx, ss, nn;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(xx) : "f"(x0), "f"(x1));
-  asm("mov.b64 %0, {%1, %1};" : "=l"(ss) : "f"(s));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(nn) : "f"(n0), "f"(n1));
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(xx) : "l"(xx), "l"(ss), "l"(nn));
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(x0), "=f"(x1) : "l"(xx));
-}
-
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]),
-      "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]),
-      "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// one query row of the output: x = o * inv as (hi, lo) 16-bit pairs [+ e4m3 cross-term views for an "f16f8" consumer GEMM]
+// two adjacent output values of one query row: (hi, lo) 16-bit pairs [+ e4m3 cross-term views for an "f16f8" consumer GEMM]
 template <int DT>
-__device__ __forceinline__ void store_row(const AttnParams& p, int b, int row, int h, const uint32_t (&o)[ATC_D], float inv) {
-  const size_t brow = (size_t)b * (p.q_batch_rows ? p.q_batch_rows : p.Lq) + row;
-  const size_t off = brow * p.ldo + h * ATC_D;
-#pragma unroll
-  for (int c8 = 0; c8 < ATC_D / 8; ++c8) {
-    uint32_t hi[4], lo[4];
-    float x[8];
-#pragma unroll
-    for (int e = 0; e < 8; ++e) x[e] = __uint_as_float(o[c8 * 8 + e]) * inv;
-#pragma unroll
-    for (int e = 0; e < 4; ++e) split2<DT>(x[2 * e], x[2 * e + 1], hi[e], lo[e]);
-    *reinterpret_cast<uint4*>(p.o_hi + off + c8 * 8) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-    if (p.o_lo) *reinterpret_cast<uint4*>(p.o_lo + off + c8 * 8) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-    if (p.o_lo8) {
-      const size_t off8 = brow * p.ldo8 + h * ATC_D + c8 * 8;
-      uint32_t l8[2], h8[2];
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const float2 f01 = __half22float2(*reinterpret_cast<const __half2*>(&hi[2 * e]));
-        const float2 f23 = __half22float2(*reinterpret_cast<const __half2*>(&hi[2 * e + 1]));
-        l8[e] = e4m3x4((x[4 * e] - f01.x) * F8_ACT_LO_SCALE, (x[4 * e + 1] - f01.y) * F8_ACT_LO_SCALE,
-                       (x[4 * e + 2] - f23.x) * F8_ACT_LO_SCALE, (x[4 * e + 3] - f23.y) * F8_ACT_LO_SCALE);
-        h8[e] = e4m3x4(x[4 * e] * F8_ACT_HI_SCALE, x[4 * e + 1] * F8_ACT_HI_SCALE, x[4 * e + 2] * F8_ACT_HI_SCALE, x[4 * e + 3] * F8_ACT_HI_SCALE);
-      }
-      *reinterpret_cast<uint2*>(p.o_lo8 + off8) = make_uint2(l8[0], l8[1]);
-      *reinterpret_cast<uint2*>(p.o_hi8 + off8) = make_uint2(h8[0], h8[1]);
-    }
+__device__ __forceinline__ void store_pair(const AttnParams& p, size_t brow, int col, float x0, float x1) {
+  uint32_t hi, lo;
+  split2<DT>(x0, x1, hi, lo);
+  const size_t off = brow * p.ldo + col;
+  *reinterpret_cast<uint32_t*>(p.o_hi + off) = hi;
+  if (p.o_lo) *reinterpret_cast<uint32_t*>(p.o_lo + off) = lo;
+  if (p.o_lo8) {
+    const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hi));
+    const size_t off8 = brow * p.ldo8 + col;
+    *reinterpret_cast<unsigned short*>(p.o_lo8 + off8) = e4m3x2((x0 - f.x) * F8_ACT_LO_SCALE, (x1 - f.y) * F8_ACT_LO_SCALE);
+    *reinterpret_cast<unsigned short*>(p.o_hi8 + off8) = e4m3x2(x0 * F8_ACT_HI_SCALE, x1 * F8_ACT_HI_SCALE);
   }
 }
 
 template <int DT>
-__global__ void __launch_bounds__(ATC_THREADS, 3) attention_tc_kernel(const __grid_constant__ AttnTcParams P) {
+__global__ void __launch_bounds__(ATC_THREADS, 2) attention_tc_kernel(const __grid_constant__ AttnTcParams P) {
   const AttnParams& p = P.a;
   extern __shared__ __align__(1024) uint8_t sm[];
   float* maskadd = reinterpret_cast<float*>(sm + OFF_MASK);
-  int* cflag = reinterpret_cast<int*>(sm + OFF_FLAG);
   uint64_t* bars = reinterpret_cast<uint64_t*>(sm + OFF_BAR);
   uint64_t* q_full = bars + 0;
   uint64_t* k_full = bars + 1;  // [2]
-  uint64_t* v_full = bars + 3;
-  uint64_t* s_full = bars + 4;  // QK(c) retired: S(c) readable
-  uint64_t* s_free = bars + 5;  // every active softmax warp has S(c) in registers
-  uint64_t* p_full = bars + 6;  // every active softmax warp has written P(c) (and finished any rescale of O)
-  uint64_t* p_free = bars + 7;  // PV(c) retired: P / V buffers reusable, O consistent
-  uint32_t* tptr = reinterpret_cast<uint32_t*>(sm + OFF_TPTR);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int wg = warp >> 2;
   const int q0 = blockIdx.x * ATC_BM, h = blockIdx.y, b = blockIdx.z;
   const int Lq = p.Lq, Lk = p.Lk;
   const int kvb = p.kv_batch_rows ? p.kv_batch_rows : Lk;
@@ -153,282 +83,179 @@ __global__ void __launch_bounds__(ATC_THREADS, 3) attention_tc_kernel(const __gr
   const int qbr = p.q_batch_rows ? p.q_batch_rows : Lq;
   const uint32_t sbase = smem_u32(sm);
   const int rows_here = min(ATC_BM, Lq - q0);
-  const int n_act = (rows_here + 31) >> 5;  // softmax warps that own at least one real query row
   const int n_all = (Lk + ATC_KC - 1) / ATC_KC;
   int n_plan = n_all;  // causal: chunks up to the tile's diagonal
   if (p.causal) {
     const int last_key = min(Lk - 1, q0 + rows_here - 1 + qp0);
     n_plan = last_key / ATC_KC + 1;
   }
-  // Pass 1 skips work that only matters for rows whose causally visible keys are all padded (chunks past the tile's diagonal, and
-  // inside the plan the chunks that are entirely hidden from a warp).  If any such skip can happen, the block votes afterwards and
-  // redoes the tile without shortcuts when some row is still "undone".
-  const bool may_rerun = p.causal && ((n_all - 1) * ATC_KC > q0 + qp0 + 31);
+  const bool may_rerun = p.causal && n_plan < n_all;
 
   if ((sbase & 1023u) != 0u) {  // the swizzled tiles assume a 1024-byte aligned window (no static shared memory in this kernel)
     if (tid == 0) printf("vima_b200: attention_tc shared memory window is not 1024-byte aligned\n");
     __trap();
   }
-  if (warp == 4) {
-    tmem_alloc<ATC_TMEM_COLS>(tptr);
-    if (lane == 0) {
-      mbar_init(q_full, 1);
-      mbar_init(&k_full[0], 1);
-      mbar_init(&k_full[1], 1);
-      mbar_init(v_full, 1);
-      mbar_init(s_full, 1);
-      mbar_init(s_free, (uint32_t)n_act);
-      mbar_init(p_full, (uint32_t)n_act);
-      mbar_init(p_free, 1);
-      fence_barrier_init();
-      tma_prefetch_desc(&P.tm_q_hi); tma_prefetch_desc(&P.tm_q_lo);
-      tma_prefetch_desc(&P.tm_k_hi); tma_prefetch_desc(&P.tm_k_lo);
-      tma_prefetch_desc(&P.tm_v_hi); tma_prefetch_desc(&P.tm_v_lo);
-    }
-  }
-  if (tid < 8) cflag[tid] = 0;
-  tcgen05_fence_before();
-  __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem = *tptr;
-
-  const uint32_t fmt = (DT == DT_BF16) ? 1u : 0u;
-  const uint32_t idesc_s = (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(ATC_KC >> 3) << 17) | ((uint32_t)(ATC_BM >> 4) << 24);
-  const uint32_t idesc_o = (1u << 4) | (fmt << 7) | (fmt << 10) | (1u << 16) | ((uint32_t)(ATC_D >> 3) << 17) | ((uint32_t)(ATC_BM >> 4) << 24);
   const int x_col = h * ATC_D;  // element column of this head inside the q / k / v row
   const int kv_row0 = b * kvb;
-
-  if (warp == 4) {
-    // =============================== control warp: lane 0 issues the TMA loads and the MMAs ===============================
-    // (the pass loop and its block-wide vote run at WARP level: an aligned barrier must be reached by the whole warp together)
-    uint32_t g = 0;                 // chunks issued so far (both passes): parity of s_* / p_* / v_full
-    uint32_t k_use[2] = {0u, 0u};   // completed fills of each K stage
-    int n = n_plan;
-    for (int pass = 0; pass < 2; ++pass) {
-      if (lane == 0) {
-        auto load_k = [&](int c, int stage) {
-          uint8_t* dst = sm + OFF_K + stage * 8192;
-          mbar_arrive_expect_tx(&k_full[stage], 8192u);
-          tma_load_2d(dst, &P.tm_k_hi, &k_full[stage], x_col, kv_row0 + c * ATC_KC);
-          tma_load_2d(dst + 4096, &P.tm_k_lo, &k_full[stage], x_col, kv_row0 + c * ATC_KC);
-        };
-        auto load_v = [&](int c) {
-          mbar_arrive_expect_tx(v_full, 8192u);
-          tma_load_2d(sm + OFF_VH, &P.tm_v_hi, v_full, x_col, kv_row0 + c * ATC_KC);
-          tma_load_2d(sm + OFF_VL, &P.tm_v_lo, v_full, x_col, kv_row0 + c * ATC_KC);
-        };
-        auto issue_qk = [&](int c, uint32_t gg) {  // gg = global index of chunk c
-          const int stage = c & 1;
-          mbar_wait(&k_full[stage], k_use[stage] & 1u);
-          k_use[stage]++;
-          if (gg > 0) mbar_wait(s_free, (gg - 1) & 1u);  // S(previous chunk) has been read out
-          tcgen05_fence_after();
-          const uint64_t dqh = desc_sw64(sbase + OFF_QH), dql = desc_sw64(sbase + OFF_QL);
-          const uint64_t dkh = desc_sw64(sbase + OFF_K + stage * 8192), dkl = desc_sw64(sbase + OFF_K + stage * 8192 + 4096);
-#pragma unroll
-          for (int k = 0; k < ATC_D / 16; ++k) umma_f16(tmem, dqh + 2 * k, dkh + 2 * k, idesc_s, (uint32_t)(k != 0));
-#pragma unroll
-          for (int k = 0; k < ATC_D / 16; ++k) umma_f16(tmem, dql + 2 * k, dkh + 2 * k, idesc_s, 1u);
-#pragma unroll
-          for (int k = 0; k < ATC_D / 16; ++k) umma_f16(tmem, dqh + 2 * k, dkl + 2 * k, idesc_s, 1u);
-          umma_commit(s_full);
-        };
-        if (pass == 0) {
-          mbar_arrive_expect_tx(q_full, 16384u);
-          tma_load_2d(sm + OFF_QH, &P.tm_q_hi, q_full, x_col, b * qbr + q0);
-          tma_load_2d(sm + OFF_QL, &P.tm_q_lo, q_full, x_col, b * qbr + q0);
-        }
-        load_k(0, 0);
-        if (n > 1) load_k(1, 1);
-        load_v(0);
-        if (pass == 0) mbar_wait(q_full, 0);
-        issue_qk(0, g);
-        for (int c = 0; c < n; ++c, ++g) {
-          if (c + 1 < n) issue_qk(c + 1, g + 1);
-          mbar_wait(p_full, g & 1u);
-          mbar_wait(v_full, g & 1u);
-          tcgen05_fence_after();
-          {
-            const uint64_t dph = desc_sw128(sbase + OFF_PH), dpl = desc_sw128(sbase + OFF_PL);
-            const uint64_t dvh = desc_sw64(sbase + OFF_VH), dvl = desc_sw64(sbase + OFF_VL);  // MN-major B: one 64-byte row per key
-            const uint32_t t_o = tmem + 64;
-#pragma unroll
-            for (int k = 0; k < ATC_KC / 16; ++k) umma_f16(t_o, dph + 2 * k, dvh + 64 * k, idesc_o, (uint32_t)((c | k) != 0));
-#pragma unroll
-            for (int k = 0; k < ATC_KC / 16; ++k) umma_f16(t_o, dpl + 2 * k, dvh + 64 * k, idesc_o, 1u);
-#pragma unroll
-            for (int k = 0; k < ATC_KC / 16; ++k) umma_f16(t_o, dph + 2 * k, dvl + 64 * k, idesc_o, 1u);
-          }
-          umma_commit(p_free);
-          mbar_wait(p_free, g & 1u);  // PV(c) -- and with it QK(c), QK(c+1) -- retired: their operand slots are free
-          if (c + 2 < n) load_k(c + 2, c & 1);
-          if (c + 1 < n) load_v(c + 1);
-        }
-      }
-      __syncwarp();
-      // every row past the causal range must have seen a valid key; otherwise the whole tile is redone over all chunks
-      if (pass == 1 || !may_rerun) break;
-      if (!__syncthreads_or(0)) break;  // vote of the softmax warps; this warp only joins the barrier
-      n = n_all;
-    }
-  } else {
-    // ======================================= softmax warps =======================================
-    // key mask row of this batch element as additive terms; per-chunk "has masked keys" flags
-    for (int j = tid; j < n_all * ATC_KC; j += 128) {
-      float mk = -INFINITY;  // beyond the sequence: excluded
-      if (j < Lk) mk = (p.key_mask == nullptr || p.key_mask[(size_t)b * mld + j]) ? 0.f : FP32_MIN_TC;
-      maskadd[j] = mk;
-      if (mk != 0.f) atomicOr(&cflag[j >> 6], 1);
-    }
-    named_bar_sync(1, 128);
-    const bool w_on = warp < n_act;
-    const int row = q0 + tid;
-    const uint32_t t_row = tmem + ((uint32_t)(warp * 32) << 16);
-    const float c_l2 = p.scale * LOG2E_TC;
-    const int rpos = row + qp0;                       // this row's key position (causal)
-    const int wpos_min = q0 + warp * 32 + qp0;        // smallest / largest key position among the warp's rows
-    const int wpos_max = wpos_min + 31;
-    // this thread's P row: 8 x 16-byte slots, 128B swizzle (slot ^ (row & 7))
-    uint32_t pslot[8];
-#pragma unroll
-    for (int c8 = 0; c8 < 8; ++c8) pslot[c8] = sbase + OFF_PH + (uint32_t)tid * 128u + (uint32_t)((c8 ^ (tid & 7)) << 4);
-    float m_ref = -INFINITY, l_run = 0.f;
-    uint32_t g = 0;
-    int n = n_plan;
-    for (int pass = 0; pass < 2; ++pass) {
-      const bool full = pass == 1;
-      if (full) { m_ref = -INFINITY; l_run = 0.f; }
-      if (w_on) {
-        for (int c = 0; c < n; ++c, ++g) {
-          const int k0 = c * ATC_KC;
-          const bool hidden = p.causal && !full && k0 > wpos_max;  // every key of the chunk is causally hidden from this warp
-          mbar_wait(s_full, g & 1u);
-          tcgen05_fence_after();
-          uint32_t ph[ATC_KC / 2], pl[ATC_KC / 2];
-          float ps = 0.f, m_use = m_ref;
-          bool grow = false;
-          if (!hidden) {
-            uint32_t sv[ATC_KC];
-            tmem_ld_32x32(t_row, *reinterpret_cast<uint32_t(*)[32]>(&sv[0]));
-            tmem_ld_32x32(t_row + 32, *reinterpret_cast<uint32_t(*)[32]>(&sv[32]));
-            tmem_ld_wait();
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(s_free);
-            const bool needs_causal = p.causal && (k0 + ATC_KC - 1 > wpos_min);
-            float mx, sc;
-            if (!needs_causal && !cflag[c]) {  // plain chunk: the scale rides in the exponent FMA
-              float m0 = __uint_as_float(sv[0]), m1 = __uint_as_float(sv[1]);
-#pragma unroll
-              for (int i = 2; i < ATC_KC; i += 4) {
-                m0 = max3(m0, __uint_as_float(sv[i]), __uint_as_float(sv[i + 1]));
-                if (i + 3 < ATC_KC) m1 = max3(m1, __uint_as_float(sv[i + 2]), __uint_as_float(sv[i + 3]));
-              }
-              mx = fmaxf(m0, m1) * c_l2;
-              sc = c_l2;
-            } else if (!needs_causal) {  // padded keys, no causal boundary in this chunk: additive mask terms, packed
-              float m0 = -INFINITY, m1 = -INFINITY;
-#pragma unroll
-              for (int c4 = 0; c4 < ATC_KC; c4 += 4) {
-                const float4 m4 = *reinterpret_cast<const float4*>(maskadd + k0 + c4);
-                float x0 = __uint_as_float(sv[c4]), x1 = __uint_as_float(sv[c4 + 1]);
-                float x2 = __uint_as_float(sv[c4 + 2]), x3 = __uint_as_float(sv[c4 + 3]);
-                fma2v(x0, x1, c_l2, m4.x, m4.y);
-                fma2v(x2, x3, c_l2, m4.z, m4.w);
-                sv[c4] = __float_as_uint(x0); sv[c4 + 1] = __float_as_uint(x1);
-                sv[c4 + 2] = __float_as_uint(x2); sv[c4 + 3] = __float_as_uint(x3);
-                m0 = max3(m0, x0, x1);
-                m1 = max3(m1, x2, x3);
-              }
-              mx = fmaxf(m0, m1);
-              sc = 1.f;
-            } else {
-              mx = -INFINITY;
-#pragma unroll
-              for (int c4 = 0; c4 < ATC_KC; c4 += 4) {
-                const float4 m4 = *reinterpret_cast<const float4*>(maskadd + k0 + c4);
-                const float mm[4] = {m4.x, m4.y, m4.z, m4.w};
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  float y = fmaf(__uint_as_float(sv[c4 + e]), c_l2, mm[e]);
-                  if (p.causal && k0 + c4 + e > rpos) y = CAUSAL_L2_TC + mm[e];
-                  sv[c4 + e] = __float_as_uint(y);
-                  mx = fmaxf(mx, y);
-                }
-              }
-              sc = 1.f;
-            }
-            grow = mx > m_ref + LAZY_THRESH;  // also the first chunk (m_ref = -inf)
-            if (grow) m_use = mx;
-            const float neg_m = -m_use;
-            float ps0 = 0.f, ps1 = 0.f;
-#pragma unroll
-            for (int i = 0; i < ATC_KC / 2; ++i) {
-              float x0 = __uint_as_float(sv[2 * i]), x1 = __uint_as_float(sv[2 * i + 1]);
-              fma2(x0, x1, sc, neg_m);
-              const float p0 = ex2_approx(x0), p1 = ex2_approx(x1);
-              ps0 += p0;
-              ps1 += p1;
-              split2<DT>(p0, p1, ph[i], pl[i]);
-            }
-            ps = ps0 + ps1;
-          } else {
-            tcgen05_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(s_free);
-#pragma unroll
-            for (int i = 0; i < ATC_KC / 2; ++i) { ph[i] = 0u; pl[i] = 0u; }
-          }
-          // the P buffer is free and O is quiescent once PV of the previous chunk has retired
-          if (g > 0) mbar_wait(p_free, (g - 1) & 1u);
-          // raise the reference maximum of the rows that need it: O and l carry exp2(-m_ref)
-          float f = 1.f;
-          if (grow && c > 0) f = ex2_approx(m_ref - m_use);
-          if (c > 0 && __any_sync(0xffffffffu, grow)) {
-            uint32_t ov[ATC_D];
-            tcgen05_fence_after();
-            tmem_ld_32x32(t_row + 64, ov);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < ATC_D; ++i) ov[i] = __float_as_uint(__uint_as_float(ov[i]) * f);
-            tmem_st_32x32(t_row + 64, ov);
-            tmem_st_wait();
-          }
-          l_run = (c > 0 ? l_run * f : 0.f) + ps;
-          m_ref = m_use;
-#pragma unroll
-          for (int c8 = 0; c8 < 8; ++c8) {
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(pslot[c8]), "r"(ph[4 * c8]), "r"(ph[4 * c8 + 1]), "r"(ph[4 * c8 + 2]),
-                         "r"(ph[4 * c8 + 3]) : "memory");
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(pslot[c8] + (uint32_t)(OFF_PL - OFF_PH)), "r"(pl[4 * c8]),
-                         "r"(pl[4 * c8 + 1]), "r"(pl[4 * c8 + 2]), "r"(pl[4 * c8 + 3]) : "memory");
-          }
-          fence_proxy_async();  // generic-proxy writes -> visible to the tensor core's async-proxy reads
-          tcgen05_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(p_full);
-        }
-        mbar_wait(p_free, (g - 1) & 1u);  // the last PV has retired: O is complete
-        tcgen05_fence_after();
-      }
-      if (pass == 1 || !may_rerun) break;
-      const int undone = w_on && row < Lq && !(m_ref > EXIT_L2_TC);
-      if (!__syncthreads_or(undone)) break;
-      n = n_all;
-    }
-    // ---- normalise and store (hi, lo) [+ e4m3 views] ----
-    if (w_on) {
-      uint32_t ov[ATC_D];
-      tmem_ld_32x32(t_row + 64, ov);
-      tmem_ld_wait();
-      if (row < Lq) store_row<DT>(p, b, row, h, ov, 1.0f / l_run);
-    }
+  if (tid == 0) {
+    mbar_init(q_full, 1);
+    mbar_init(&k_full[0], 1);
+    mbar_init(&k_full[1], 1);
+    fence_barrier_init();
+    tma_prefetch_desc(&P.tm_q_hi); tma_prefetch_desc(&P.tm_q_lo);
+    tma_prefetch_desc(&P.tm_k_hi); tma_prefetch_desc(&P.tm_k_lo);
   }
-  tcgen05_fence_before();
+  // key mask row of this batch element as additive terms
+  for (int j = tid; j < n_all * ATC_KC; j += ATC_THREADS) {
+    float mk = -INFINITY;  // beyond the sequence: excluded
+    if (j < Lk) mk = (p.key_mask == nullptr || p.key_mask[(size_t)b * mld + j]) ? 0.f : FP32_MIN_TC;
+    maskadd[j] = mk;
+  }
   __syncthreads();
-  if (warp == 4) {
-    tcgen05_fence_after();
-    tmem_dealloc<ATC_TMEM_COLS>(tmem);
+
+  auto load_k = [&](int c, int stage) {  // thread 0 only
+    uint8_t* dst = sm + OFF_K + stage * 8192;
+    mbar_arrive_expect_tx(&k_full[stage], 8192u);
+    tma_load_2d(dst, &P.tm_k_hi, &k_full[stage], x_col, kv_row0 + c * ATC_KC);
+    tma_load_2d(dst + 4096, &P.tm_k_lo, &k_full[stage], x_col, kv_row0 + c * ATC_KC);
+  };
+  if (tid == 0) {
+    mbar_arrive_expect_tx(q_full, 16384u);
+    tma_load_2d(sm + OFF_QH, &P.tm_q_hi, q_full, x_col, b * qbr + q0);
+    tma_load_2d(sm + OFF_QL, &P.tm_q_lo, q_full, x_col, b * qbr + q0);
+  }
+
+  // accumulator fragment rows of this thread: r_loc + 8*hh (hh = 0, 1) inside the tile; columns 8*g + 2*qd + (0, 1)
+  const int r_loc = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int qd = lane & 3;
+  const float c_l2 = p.scale * LOG2E_TC;
+  const uint64_t dqh = wgmma_desc_sw64(sbase + OFF_QH + wg * 4096), dql = wgmma_desc_sw64(sbase + OFF_QL + wg * 4096);
+  // this thread's share of a V chunk: key vj, dims 8*vd .. 8*vd+7 (hi and lo)
+  const int vj = tid >> 2, vd = tid & 3;
+  uint32_t k_use[2] = {0u, 0u};  // completed fills of each K stage
+  float o[16], m_run[2], l_run[2];
+  int n = n_plan;
+  for (int pass = 0; pass < 2; ++pass) {
+#pragma unroll
+    for (int i = 0; i < 16; ++i) o[i] = 0.f;
+    m_run[0] = m_run[1] = -INFINITY;
+    l_run[0] = l_run[1] = 0.f;
+    if (tid == 0) {
+      load_k(0, 0);
+      if (n > 1) load_k(1, 1);
+    }
+    if (pass == 0) mbar_wait(q_full, 0);
+    for (int c = 0; c < n; ++c) {
+      const int stage = c & 1;
+      const int k0 = c * ATC_KC;
+      mbar_wait(&k_full[stage], k_use[stage] & 1u);
+      k_use[stage]++;
+      float s[32];
+      {
+        const uint64_t dkh = wgmma_desc_sw64(sbase + OFF_K + stage * 8192), dkl = wgmma_desc_sw64(sbase + OFF_K + stage * 8192 + 4096);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < ATC_D / 16; ++k) wgmma_m64n64k16_ss<DT>(s, dqh + 2 * k, dkh + 2 * k, (uint32_t)(k != 0));
+#pragma unroll
+        for (int k = 0; k < ATC_D / 16; ++k) wgmma_m64n64k16_ss<DT>(s, dql + 2 * k, dkh + 2 * k, 1u);
+#pragma unroll
+        for (int k = 0; k < ATC_D / 16; ++k) wgmma_m64n64k16_ss<DT>(s, dqh + 2 * k, dkl + 2 * k, 1u);
+        wgmma_commit();
+      }
+      // V(c) -> V^T tile (dim n, key k at n*128 + (((k>>3) ^ (n&7)) << 4) + (k&7)*2), while the tensor cores work on S
+      {
+        uint4 vh = make_uint4(0u, 0u, 0u, 0u), vl = vh;
+        if (k0 + vj < Lk) {
+          const size_t off = (size_t)(kv_row0 + k0 + vj) * p.ldv + x_col + vd * 8;
+          vh = __ldg(reinterpret_cast<const uint4*>(p.v_hi + off));
+          vl = __ldg(reinterpret_cast<const uint4*>(p.v_lo + off));
+        }
+        uint8_t* vt = sm + OFF_VT + stage * 8192;
+        const uint32_t wh[4] = {vh.x, vh.y, vh.z, vh.w}, wl[4] = {vl.x, vl.y, vl.z, vl.w};
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+          const int nn = vd * 8 + e;
+          const int off = nn * 128 + ((((vj >> 3) ^ (nn & 7))) << 4) + (vj & 7) * 2;
+          *reinterpret_cast<unsigned short*>(vt + off) = (unsigned short)(wh[e >> 1] >> (16 * (e & 1)));
+          *reinterpret_cast<unsigned short*>(vt + 4096 + off) = (unsigned short)(wl[e >> 1] >> (16 * (e & 1)));
+        }
+        fence_proxy_async();  // generic-proxy writes -> visible to the tensor core's async-proxy reads
+      }
+      wgmma_wait<0>();
+      wgmma_fence_acc(s);
+      // ---- softmax on the fragment: element 4g+e is row r_loc + 8*(e>>1), key k0 + 8g + 2qd + (e&1) ----
+      float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+      for (int g = 0; g < 8; ++g)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int key = k0 + 8 * g + 2 * qd + (e & 1);
+          const float mm = maskadd[key];
+          float y = fmaf(s[4 * g + e], c_l2, mm);
+          if (p.causal && key > q0 + r_loc + 8 * (e >> 1) + qp0) y = CAUSAL_L2_TC + mm;
+          s[4 * g + e] = y;
+          mx[e >> 1] = fmaxf(mx[e >> 1], y);
+        }
+      float f[2];
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 1));
+        mx[hh] = fmaxf(mx[hh], __shfl_xor_sync(0xffffffffu, mx[hh], 2));
+        const float m_new = fmaxf(m_run[hh], mx[hh]);
+        f[hh] = ex2_approx(m_run[hh] - m_new);  // 0 on the first chunk (m_run = -inf)
+        m_run[hh] = m_new;
+      }
+      uint32_t ph[16], pl[16];
+      float ps[2] = {0.f, 0.f};
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {  // pair i = elements 2i, 2i+1: row half (i & 1)
+        const int hh = i & 1;
+        const float p0 = ex2_approx(s[2 * i] - m_run[hh]), p1 = ex2_approx(s[2 * i + 1] - m_run[hh]);
+        ps[hh] += p0 + p1;
+        split2<DT>(p0, p1, ph[i], pl[i]);
+      }
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) l_run[hh] = l_run[hh] * f[hh] + ps[hh];
+#pragma unroll
+      for (int i = 0; i < 16; ++i) o[i] *= f[(i >> 1) & 1];
+      // V^T(c) is complete, and both warpgroups are done reading K(c): its slot takes K(c+2)
+      named_bar_sync(1, ATC_THREADS);
+      if (tid == 0 && c + 2 < n) load_k(c + 2, stage);
+      {
+        const uint64_t dvh = wgmma_desc_sw128(sbase + OFF_VT + stage * 8192), dvl = wgmma_desc_sw128(sbase + OFF_VT + stage * 8192 + 4096);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < ATC_KC / 16; ++kk) {  // A fragment of keys [16kk, +16): pairs 4kk .. 4kk+3
+          const uint32_t ah[4] = {ph[4 * kk], ph[4 * kk + 1], ph[4 * kk + 2], ph[4 * kk + 3]};
+          const uint32_t al[4] = {pl[4 * kk], pl[4 * kk + 1], pl[4 * kk + 2], pl[4 * kk + 3]};
+          wgmma_m64n32k16_rs<DT>(o, ah, dvh + 2 * kk, 1u);
+          wgmma_m64n32k16_rs<DT>(o, al, dvh + 2 * kk, 1u);
+          wgmma_m64n32k16_rs<DT>(o, ah, dvl + 2 * kk, 1u);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_acc(o);
+      }
+    }
+    // every row past the causal range must have seen a valid key; otherwise the whole tile is redone over all chunks
+    if (pass == 1 || !may_rerun) break;
+    const int undone = (r_loc < rows_here && !(m_run[0] > EXIT_L2_TC)) || (r_loc + 8 < rows_here && !(m_run[1] > EXIT_L2_TC));
+    if (!__syncthreads_or(undone)) break;
+    n = n_all;
+  }
+  // ---- normalise and store (hi, lo) [+ e4m3 views] ----
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    float l = l_run[hh];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const int row = q0 + r_loc + 8 * hh;
+    if (row < Lq) {
+      const float inv = 1.0f / l;
+      const size_t brow = (size_t)b * qbr + row;
+#pragma unroll
+      for (int g = 0; g < 4; ++g) store_pair<DT>(p, brow, x_col + 8 * g + 2 * qd, o[4 * g + 2 * hh] * inv, o[4 * g + 2 * hh + 1] * inv);
+    }
   }
 }
 
@@ -470,9 +297,7 @@ cudaError_t launch_attention_tc(const AttnParams& p, void* encode_fn, cudaStream
   bool ok = make_map(encode_fn, &P.tm_q_hi, p.q_hi, p.dtype, (long long)p.B * qbr, cols, p.ldq, ATC_BM) &&
             make_map(encode_fn, &P.tm_q_lo, p.q_lo, p.dtype, (long long)p.B * qbr, cols, p.ldq, ATC_BM) &&
             make_map(encode_fn, &P.tm_k_hi, p.k_hi, p.dtype, (long long)p.B * kvb, cols, p.ldk, ATC_KC) &&
-            make_map(encode_fn, &P.tm_k_lo, p.k_lo, p.dtype, (long long)p.B * kvb, cols, p.ldk, ATC_KC) &&
-            make_map(encode_fn, &P.tm_v_hi, p.v_hi, p.dtype, (long long)p.B * kvb, cols, p.ldv, ATC_KC) &&
-            make_map(encode_fn, &P.tm_v_lo, p.v_lo, p.dtype, (long long)p.B * kvb, cols, p.ldv, ATC_KC);
+            make_map(encode_fn, &P.tm_k_lo, p.k_lo, p.dtype, (long long)p.B * kvb, cols, p.ldk, ATC_KC);
   if (!ok) return cudaErrorInvalidValue;
   dim3 grid((p.Lq + ATC_BM - 1) / ATC_BM, p.H, p.B);
   const size_t smem = ATC_SMEM;

@@ -1,17 +1,15 @@
-// tcgen05 GEMM for sm_100a:  C[M,N] = epilogue( A[M,K] * B[N,K]^T )
+// wgmma GEMM for sm_90a:  C[M,N] = epilogue( A[M,K] * B[N,K]^T )
 //
 //  * A (activations) and B (packed weights) are K-major 16-bit operands (fp16 or bf16), optionally as (hi, lo)
-//    pairs: in split mode the kernel accumulates A_hi*B_hi + A_lo*B_hi + A_hi*B_lo in the SAME fp32 TMEM
+//    pairs: in split mode the kernel accumulates A_hi*B_hi + A_lo*B_hi + A_hi*B_lo in the SAME fp32 register
 //    accumulator, which restores ~fp32 products (see DESIGN.md "operand precision").
-//  * Persistent, warp-specialised: warp 0 = TMA producer, warp 1 = MMA issuer (one elected lane),
-//    warp 2 = TMEM allocator, warps 4..7 = epilogue (TMEM -> registers -> smem transpose -> 128-bit coalesced global).
+//  * Persistent, warp-specialised: warps 0-7 = two consumer warpgroups (rows [0,64) and [64,128) of the 128-row tile; each
+//    issues its wgmma M64 N64 instructions and runs the epilogue of its rows), warp 8 = TMA producer (one lane).
 //  * smem ring of `n_stages` stages {A_hi,[A_lo],B_hi,[B_lo]} in the 128-byte swizzled K-major layout that TMA
-//    writes and the UMMA descriptors read; two 256-column fp32 accumulators in TMEM so the epilogue of tile i
-//    overlaps the main loop of tile i+1.
+//    writes and the wgmma descriptors read; the producer fills the next tile's stages while the consumers run the epilogue.
 //  * Epilogue: acc*scale + bias -> activation -> (GLU pair product) -> *mul -> +residual -> fp32 and/or (hi,lo).
 //    The epilogue is specialised at compile time (EpiCfg) for the combinations the VIMA path uses; a generic
-//    runtime-flag variant covers everything else.  v0 of this kernel was epilogue-bound by 10x (scalar 2-byte
-//    stores, runtime flag tests per element: profiles/r1_gemm_v0_epilogue_bound.csv).
+//    runtime-flag variant covers everything else.
 #pragma once
 #include "common.cuh"
 
@@ -20,23 +18,22 @@ namespace vima {
 constexpr int GEMM_BM = 128;
 constexpr int GEMM_BK = 64;                       // 64 x 2 B = 128 B = one swizzle row
 constexpr int GEMM_A_TILE_BYTES = GEMM_BM * 128;  // 16 KB
-constexpr int GEMM_THREADS = 384;       // 4 control warps (TMA, MMA, TMEM alloc, spare) + 8 epilogue warps
-constexpr int GEMM_EPI_WARPS = 8;       // two per TMEM lane quadrant: each takes every other 32-column chunk
+constexpr int GEMM_CONSUMERS = 256;               // two warpgroups
+constexpr int GEMM_THREADS = GEMM_CONSUMERS + 32; // + the TMA producer warp
+constexpr int GEMM_MAX_BN = 128;                  // two 64-column accumulator chunks per thread (64 fp32 registers): with 9 warps
+                                                  // per CTA one SM sub-partition holds 3 of them, which caps a thread at 168 registers
 constexpr int GEMM_MAX_STAGES = 8;
-constexpr int GEMM_STAGING_BYTES = GEMM_EPI_WARPS * 32 * 16 * 4;  // per-epilogue-warp 32x16 fp32 transpose buffers (XOR-swizzled)
-constexpr int GEMM_TMEM_COLS = 512;
+constexpr int GEMM_STAGING_BYTES = 8 * 16 * 16 * 4;  // per-consumer-warp 16x16 fp32 transpose buffers (XOR-swizzled)
 
 struct alignas(64) GemmParams {
   CUtensorMap tm_a_hi, tm_a_lo, tm_b_hi, tm_b_lo;  // in mode 2: tm_a_lo = A_lo8, tm_b_lo = B_lo8
   CUtensorMap tm_a_hi8, tm_b_hi8;                    // mode 2 only
   int M, N, K;      // N = accumulator columns (2x the output columns in GLU mode)
-  int block_n;      // multiple of 32 (64 in GLU mode), <= 256
+  int block_n;      // multiple of 32 (64 in GLU mode), <= GEMM_MAX_BN
   int n_stages;
-  int mcast;        // 1: launched as 2-CTA clusters; the pair shares one B tile (each CTA TMA-multicasts half of it)
-  int two_cta;      // 1: launched as 2-CTA clusters running cta_group::2 MMAs (M = 256 per pair; each CTA holds half of B)
   int split;        // 0: hi*hi only, 1: three-term fp16 split product, 2: fp16 hi*hi + two fp8 cross terms
   int dtype;        // DT_F16 / DT_BF16 (operand and 16-bit output format)
-  int epi_prefetch; // 1: epilogue warps pull the next tile's residual / multiplier rows into L2 one tile ahead
+  int epi_prefetch; // 1: consumer warps pull the next tile's residual / multiplier rows into L2 one tile ahead
   int glu;          // 1: out[:, t*bn/2 + c] = act(acc[c]+bias[c]) * (acc[bn/2+c]+bias[bn/2+c]) per tile t
   int act;
   float acc_scale;  // un-scale of pre-scaled packed weights (power of two)
@@ -80,18 +77,7 @@ struct EpiCfg {
   static constexpr bool STATS = STATS_;  // emit per-row partial (sum, sum of squares) of the output
 };
 
-constexpr int GEMM_COLVEC_PLANES = 4;  // per accumulator buffer: bias | ln_c1 | res_gamma | res_beta, 256 floats each
-
-__device__ __forceinline__ uint64_t make_sw128_kmajor_desc(uint32_t smem_addr) {
-  // start address [0,14) (>>4) | LBO [16,30) (ignored for swizzled K-major; 1) | SBO [32,46) = 8 rows * 128 B
-  // | version [46,48) = 1 (sm_100) | layout type [61,64) = 2 (SWIZZLE_128B)
-  return (uint64_t)((smem_addr >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-
-__device__ __forceinline__ uint64_t make_sw64_kmajor_desc(uint32_t smem_addr) {
-  // fp8 tiles: rows of 64 bytes (64 K-elements), SWIZZLE_64B (layout type 4), SBO = 8 rows * 64 B
-  return (uint64_t)((smem_addr >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)(512 >> 4) << 32) | (1ull << 46) | (4ull << 61);
-}
+constexpr int GEMM_COLVEC_PLANES = 4;  // per buffer: bias | ln_c1 | res_gamma | res_beta, 256 floats each
 
 template <int ACT>
 __device__ __forceinline__ float act_ct(float x) {
@@ -105,14 +91,24 @@ __device__ __forceinline__ float act_ct(float x) {
 template <int DT>
 __device__ __forceinline__ void split4(const float4& y, uint2& hi, uint2& lo) { split4v<DT>(y, hi, lo); }
 
-// One accumulator tile, this warp's share: rows [32*quadrant, +32) x every other 32-column chunk (ehalf selects which).
-// Per 16-column sub-chunk: TMEM -> registers (row per thread) -> bias/act/GLU -> smem transpose (32x16 floats, 16-byte chunks
-// XOR-swizzled by (row>>1)&3: conflict-free both ways) -> [8 rows x 4 lanes x float4] -> mul / residual / stores (128-bit fp32,
-// 64-bit 16-bit pairs), issued after the sub-chunk's global loads are already in flight.
+// the 8 accumulator values of 16-column group s (columns 16s .. 16s+15) of this thread: the gate half of a GLU tile sits at a
+// run-time offset (block_n / 2), so its group index is only known at run time
+__device__ __forceinline__ void acc_group16(const float (&acc)[GEMM_MAX_BN / 64][32], int s, float (&v)[8]) {
+#pragma unroll
+  for (int t = 0; t < GEMM_MAX_BN / 16; ++t)
+    if (t == s) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) v[i] = acc[t >> 2][(t & 3) * 8 + i];
+    }
+}
+
+// One accumulator tile, this warp's share: rows [row_base, +16) x every column.  Per 16-column sub-chunk: fragment registers
+// -> bias/act/GLU -> smem transpose (16x16 floats, 16-byte chunks XOR-swizzled by (row>>1)&3) -> [8 rows x 4 lanes x float4]
+// -> mul / residual / stores (128-bit fp32, 64-bit 16-bit pairs), issued after the sub-chunk's global loads are already in flight.
+// Row statistics keep the two column halves of the original layout: part 2*tn + ((column / 32) & 1).
 template <class E>
-__device__ __forceinline__ void epilogue_tile(const GemmParams& p, uint32_t t_row, const float* __restrict__ sb, float* __restrict__ st,
-                                              int lane, int ehalf, int row_base, int tn, int bn_out, int n_out, uint64_t* acc_full,
-                                              uint32_t acc_phase) {
+__device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float (&acc)[GEMM_MAX_BN / 64][32], const float* __restrict__ sb,
+                                              float* __restrict__ st, int lane, int row_base, int tn, int bn_out, int n_out) {
   const bool glu = E::GENERIC ? (p.glu != 0) : E::GLU;
   const bool has_mul = E::GENERIC ? (p.mul != nullptr) : E::MUL;
   const bool has_res = E::GENERIC ? (p.residual != nullptr) : E::RES;
@@ -122,26 +118,30 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, uint32_t t_ro
   const bool lnr = E::GENERIC ? (p.res_stats != nullptr) : E::LNR;
   const bool stats = E::GENERIC ? (p.stats_out != nullptr) : E::STATS;
   const float scale = p.acc_scale;
-  const int sub = lane >> 2;        // row within a group of 8
-  const int kc = lane & 3;          // which 4-column group of the 16-column sub-chunk
+  const int sub = lane >> 2;        // row within a group of 8 (transposed layout); also the fragment row
+  const int kc = lane & 3;          // which 4-column group of the 16-column sub-chunk; also the fragment column pair
   const float* sc1 = sb + 256;      // ln_c1 tile (accumulator-column order, like the bias tile)
   const float* sgam = sb + 512;     // res_gamma / res_beta tiles (output-column order)
   const float* sbet = sb + 768;
-  // folded LayerNorm of the A rows: this thread's accumulator row is `row_base + lane`
-  float a_mean = 0.f, a_rstd = 1.f;
+  // folded LayerNorm of the A rows: this thread's fragment rows are row_base + sub + 8*h
+  float a_mean[2] = {0.f, 0.f}, a_rstd[2] = {1.f, 1.f};
   if (lna) {
-    const int row = row_base + lane;
-    if (row < p.M) {
-      const float2 ms = __ldg(reinterpret_cast<const float2*>(p.row_stats) + row);
-      a_mean = ms.x; a_rstd = ms.y;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = row_base + sub + 8 * h;
+      if (row < p.M) {
+        const float2 ms = __ldg(reinterpret_cast<const float2*>(p.row_stats) + row);
+        a_mean[h] = ms.x; a_rstd[h] = ms.y;
+      }
     }
   }
   const bool ln_gate = lna && p.ln_cols == 1;
   // on-the-fly LayerNorm of the residual rows / partial output statistics: rows it*8 + sub of the transposed layout
-  float r_mean[4], r_rstd[4], st1[4], st2[4];
+  float r_mean[2], r_rstd[2], st1[2][2], st2[2][2];
 #pragma unroll
-  for (int it = 0; it < 4; ++it) {
-    r_mean[it] = 0.f; r_rstd[it] = 1.f; st1[it] = 0.f; st2[it] = 0.f;
+  for (int it = 0; it < 2; ++it) {
+    r_mean[it] = 0.f; r_rstd[it] = 1.f;
+    st1[0][it] = st1[1][it] = st2[0][it] = st2[1][it] = 0.f;
     if (lnr) {
       const int row = row_base + it * 8 + sub;
       if (row < p.M) {
@@ -150,104 +150,69 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, uint32_t t_ro
       }
     }
   }
-  // This warp's 16-column sub-chunks: s -> columns ehalf*32 + (s/2)*64 + (s%2)*16.  The multiplier / residual rows of sub-chunk
-  // s+1 are requested before sub-chunk s is processed (one sub-chunk of register prefetch): their latency -- the largest single
-  // stall of the residual-carrying N = 768 GEMMs in the round-2 ncu source view -- overlaps the TMEM read, the transpose and the
-  // stores of the sub-chunk in hand.
-  const int n_sub = ((bn_out - ehalf * 32 + 63) / 64) * 2;
-  auto sub_j = [&](int s) { return ehalf * 32 + (s >> 1) * 64 + (s & 1) * 16; };
-  auto load_mr = [&](int j, float4 (&mm_)[4], float4 (&rr_)[4]) {
+  auto load_mr = [&](int j, float4 (&mm_)[2], float4 (&rr_)[2]) {
     const int col = tn * bn_out + j + kc * 4;
     const bool col_ok = col < n_out;
 #pragma unroll
-    for (int it = 0; it < 4; ++it) {
+    for (int it = 0; it < 2; ++it) {
       const int row = row_base + it * 8 + sub;
       const bool ok = col_ok && row < p.M;
       if (has_mul) mm_[it] = ok ? __ldg(reinterpret_cast<const float4*>(p.mul + (size_t)row * p.ld_mul + col)) : make_float4(1.f, 1.f, 1.f, 1.f);
       if (has_res) rr_[it] = ok ? __ldg(reinterpret_cast<const float4*>(p.residual + (size_t)row * p.ld_res + col)) : make_float4(0.f, 0.f, 0.f, 0.f);
     }
   };
-  float4 mm[4], rr[4], mm_n[4], rr_n[4];
-  if (n_sub > 0) load_mr(sub_j(0), mm, rr);  // in flight while the accumulator tile is still being produced
-  mbar_wait(acc_full, acc_phase);
-  tcgen05_fence_after();
-  {
-#pragma unroll 1
-    for (int s = 0; s < n_sub; ++s) {
-      const int j = sub_j(s);
+  // The multiplier / residual rows of sub-chunk s+1 are requested before sub-chunk s is processed (one sub-chunk of register
+  // prefetch), so their latency overlaps the arithmetic, the transpose and the stores of the sub-chunk in hand.
+  float4 mm[2], rr[2], mm_n[2], rr_n[2];
+  load_mr(0, mm, rr);
+  const int wsw = (sub >> 1) & 3;  // transpose swizzle of this thread's fragment rows (sub and sub + 8 share it)
+#pragma unroll
+  for (int s = 0; s < GEMM_MAX_BN / 16; ++s) {
+    const int j = s * 16;
+    if (j < bn_out) {
       const int col = tn * bn_out + j + kc * 4;
       const bool col_ok = col < n_out;  // n_out % 4 == 0 (checked on the host)
-      if (s + 1 < n_sub) load_mr(sub_j(s + 1), mm_n, rr_n);
-      uint32_t v[16];
-      tmem_ld_32x16(t_row + j, v);
-      float x[16];
-      if (glu) {
-        uint32_t g[16];
-        tmem_ld_32x16(t_row + bn_out + j, g);
-        tmem_ld_wait();
+      if (j + 16 < bn_out) load_mr(j + 16, mm_n, rr_n);
+      float v[8], g[8], x[8];
 #pragma unroll
-        for (int i = 0; i < 16; i += 4) {
-          const float4 b1 = *reinterpret_cast<const float4*>(sb + j + i);
-          const float4 b2 = *reinterpret_cast<const float4*>(sb + bn_out + j + i);
-          const float bb1[4] = {b1.x, b1.y, b1.z, b1.w}, bb2[4] = {b2.x, b2.y, b2.z, b2.w};
+      for (int i = 0; i < 8; ++i) v[i] = acc[s >> 2][(s & 3) * 8 + i];
+      if (glu) acc_group16(acc, s + bn_out / 16, g);
+      // fragment element i: row sub + 8*((i>>1)&1), column j + 8*(i>>2) + 2*kc + (i&1)
 #pragma unroll
-          float cc1[4] = {0.f, 0.f, 0.f, 0.f}, cc2[4] = {0.f, 0.f, 0.f, 0.f};
-          if (lna) {
-            const float4 c1 = *reinterpret_cast<const float4*>(sc1 + j + i);
-            cc1[0] = c1.x; cc1[1] = c1.y; cc1[2] = c1.z; cc1[3] = c1.w;
-            if (ln_gate) {
-              const float4 c2 = *reinterpret_cast<const float4*>(sc1 + bn_out + j + i);
-              cc2[0] = c2.x; cc2[1] = c2.y; cc2[2] = c2.z; cc2[3] = c2.w;
-            }
-          }
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            float a, gt;
-            if (lna) {
-              a = fmaf(fmaf(-a_mean, cc1[q], __uint_as_float(v[i + q]) * scale), a_rstd, bb1[q]);
-              gt = ln_gate ? fmaf(fmaf(-a_mean, cc2[q], __uint_as_float(g[i + q]) * scale), a_rstd, bb2[q])
-                           : fmaf(__uint_as_float(g[i + q]), scale, bb2[q]);
-            } else {
-              a = fmaf(__uint_as_float(v[i + q]), scale, bb1[q]);
-              gt = fmaf(__uint_as_float(g[i + q]), scale, bb2[q]);
-            }
-            a = E::GENERIC ? apply_act(p.act, a) : act_ct<E::ACT>(a);
-            x[i + q] = a * gt;
-          }
-        }
-      } else {
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 16; i += 4) {
-          const float4 b1 = *reinterpret_cast<const float4*>(sb + j + i);
-          const float bb1[4] = {b1.x, b1.y, b1.z, b1.w};
-#pragma unroll
-          float cc1[4] = {0.f, 0.f, 0.f, 0.f};
-          if (lna) {
-            const float4 c1 = *reinterpret_cast<const float4*>(sc1 + j + i);
-            cc1[0] = c1.x; cc1[1] = c1.y; cc1[2] = c1.z; cc1[3] = c1.w;
-          }
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const float a = lna ? fmaf(fmaf(-a_mean, cc1[q], __uint_as_float(v[i + q]) * scale), a_rstd, bb1[q])
-                                : fmaf(__uint_as_float(v[i + q]), scale, bb1[q]);
-            x[i + q] = E::GENERIC ? apply_act(p.act, a) : act_ct<E::ACT>(a);
-          }
+      for (int i = 0; i < 8; ++i) {
+        const int c = j + 8 * (i >> 2) + 2 * kc + (i & 1);
+        const int h = (i >> 1) & 1;
+        float a;
+        if (lna) a = fmaf(fmaf(-a_mean[h], sc1[c], v[i] * scale), a_rstd[h], sb[c]);
+        else a = fmaf(v[i], scale, sb[c]);
+        if (glu) {
+          float gt;
+          if (ln_gate) gt = fmaf(fmaf(-a_mean[h], sc1[bn_out + c], g[i] * scale), a_rstd[h], sb[bn_out + c]);
+          else gt = fmaf(g[i], scale, sb[bn_out + c]);
+          a = E::GENERIC ? apply_act(p.act, a) : act_ct<E::ACT>(a);
+          x[i] = a * gt;
+        } else {
+          x[i] = E::GENERIC ? apply_act(p.act, a) : act_ct<E::ACT>(a);
         }
       }
-      const int wsw = (lane >> 1) & 3;  // this thread's row is `lane`
 #pragma unroll
-      for (int k = 0; k < 4; ++k)
-        *reinterpret_cast<float4*>(st + lane * 16 + ((k ^ wsw) << 2)) = make_float4(x[4 * k], x[4 * k + 1], x[4 * k + 2], x[4 * k + 3]);
+      for (int q = 0; q < 2; ++q)     // column group 8q .. 8q+7: 16-byte chunk 2q + kc/2, float2 at (2*kc) % 4
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = sub + 8 * h;
+          const int ch = (2 * q + (kc >> 1)) ^ wsw;
+          *reinterpret_cast<float2*>(st + r * 16 + ch * 4 + (2 * kc & 3)) = make_float2(x[4 * q + 2 * h], x[4 * q + 2 * h + 1]);
+        }
       __syncwarp();
-      float4 y[4];
+      float4 y[2];
 #pragma unroll
-      for (int it = 0; it < 4; ++it) {
+      for (int it = 0; it < 2; ++it) {
         const int r = it * 8 + sub;
         y[it] = *reinterpret_cast<const float4*>(st + r * 16 + ((kc ^ ((r >> 1) & 3)) << 2));
       }
+      const int half = (j >> 5) & 1;
 #pragma unroll
-      for (int it = 0; it < 4; ++it) {
+      for (int it = 0; it < 2; ++it) {
         const int row = row_base + it * 8 + sub;
         if (!(col_ok && row < p.M)) continue;
         float4 o = y[it];
@@ -264,8 +229,8 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, uint32_t t_ro
           o.x += r.x; o.y += r.y; o.z += r.z; o.w += r.w;
         }
         if (stats) {
-          st1[it] += (o.x + o.y) + (o.z + o.w);
-          st2[it] += fmaf(o.x, o.x, o.y * o.y) + fmaf(o.z, o.z, o.w * o.w);
+          st1[half][it] += (o.x + o.y) + (o.z + o.w);
+          st2[half][it] += fmaf(o.x, o.x, o.y * o.y) + fmaf(o.z, o.z, o.w * o.w);
         }
         if (o32) *reinterpret_cast<float4*>(p.out_f32 + (size_t)row * p.ld_o32 + col) = o;
         if (o16) {
@@ -290,48 +255,43 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, uint32_t t_ro
       }
       __syncwarp();
 #pragma unroll
-      for (int it = 0; it < 4; ++it) {
+      for (int it = 0; it < 2; ++it) {
         if (has_mul) mm[it] = mm_n[it];
         if (has_res) rr[it] = rr_n[it];
       }
     }
   }
   if (stats) {
-    // every row's 4 column-group lanes hold partial sums over this warp's chunks: fold them (fixed order -> run-to-run and
-    // batch-slice deterministic) and let the kc == 0 lane write the (n-tile, epilogue-half) partial
-    const int part = tn * 2 + ehalf;
+    // every row's 4 column-group lanes hold partial sums over its half of the columns: fold them (fixed order -> run-to-run and
+    // batch-slice deterministic) and let the kc == 0 lane write the (n-tile, half) partials
 #pragma unroll
-    for (int it = 0; it < 4; ++it) {
-      float s1 = st1[it], s2 = st2[it];
-      s1 += __shfl_xor_sync(0xffffffffu, s1, 1); s2 += __shfl_xor_sync(0xffffffffu, s2, 1);
-      s1 += __shfl_xor_sync(0xffffffffu, s1, 2); s2 += __shfl_xor_sync(0xffffffffu, s2, 2);
-      const int row = row_base + it * 8 + sub;
-      if (kc == 0 && row < p.M) reinterpret_cast<float2*>(p.stats_out)[(size_t)row * p.stats_parts + part] = make_float2(s1, s2);
-    }
+    for (int hf = 0; hf < 2; ++hf)
+#pragma unroll
+      for (int it = 0; it < 2; ++it) {
+        float s1 = st1[hf][it], s2 = st2[hf][it];
+        s1 += __shfl_xor_sync(0xffffffffu, s1, 1); s2 += __shfl_xor_sync(0xffffffffu, s2, 1);
+        s1 += __shfl_xor_sync(0xffffffffu, s1, 2); s2 += __shfl_xor_sync(0xffffffffu, s2, 2);
+        const int row = row_base + it * 8 + sub;
+        if (kc == 0 && row < p.M) reinterpret_cast<float2*>(p.stats_out)[(size_t)row * p.stats_parts + tn * 2 + hf] = make_float2(s1, s2);
+      }
   }
 }
 
-// TWO_CTA instantiations contain cta_group::2 instructions and MUST be launched as 2-CTA clusters; the others run as single
-// CTAs or (p.mcast) as 2-CTA clusters that only share the B tile by TMA multicast.
-template <class E, bool TWO_CTA>
+template <class E>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve: [stages][staging][bias 2x256 f32][barriers][tmem ptr]
+  // carve: [stages][staging][column vectors 2 x 4 x 256 f32][barriers]
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   const int BN = p.block_n;
-  constexpr int tc = TWO_CTA ? 1 : 0;
-  const int b_tile_bytes = (tc ? BN / 2 : BN) * 128;  // cta_group::2: this CTA stages only its half of the B tile
+  const int b_tile_bytes = BN * 128;
   const int n_parts = p.split ? 2 : 1;  // mode 2: the second "part" holds the two half-size fp8 tiles of each operand
   const int stage_bytes = (GEMM_A_TILE_BYTES + b_tile_bytes) * n_parts;
   uint8_t* stages = smem;
   float* staging = (float*)(smem + (size_t)p.n_stages * stage_bytes);
-  float* sbias = staging + GEMM_STAGING_BYTES / 4;  // [2 accumulator buffers][GEMM_COLVEC_PLANES][256]
+  float* sbias = staging + GEMM_STAGING_BYTES / 4;  // [2 buffers][GEMM_COLVEC_PLANES][256]
   uint64_t* bars = (uint64_t*)(sbias + 2 * GEMM_COLVEC_PLANES * 256);
-  uint64_t* full_bar = bars;                          // [n_stages]
-  uint64_t* empty_bar = bars + GEMM_MAX_STAGES;       // [n_stages]
-  uint64_t* tmem_full = bars + 2 * GEMM_MAX_STAGES;   // [2]
-  uint64_t* tmem_empty = tmem_full + 2;               // [2]
-  uint32_t* tmem_ptr_smem = (uint32_t*)(tmem_empty + 2);
+  uint64_t* full_bar = bars;                     // [n_stages]
+  uint64_t* empty_bar = bars + GEMM_MAX_STAGES;  // [n_stages]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -339,18 +299,9 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
   const int tiles_m = (p.M + GEMM_BM - 1) / GEMM_BM;
   const int tiles_n = (p.N + BN - 1) / BN;
   const int num_kb = (p.K + GEMM_BK - 1) / GEMM_BK;
-  // Work units: single tiles, or (mcast) PAIRS of vertically adjacent tiles (m_blk = 2*pair_m + rank, same n) handled by the
-  // two CTAs of a cluster so that one B tile feeds both.  A CTA whose m-block falls off the end runs a ghost tile (zero-filled
-  // loads, no stores) to keep the pair's barrier protocol in step.
-  const int mc = p.mcast;
-  const bool paired = mc || tc;
-  const uint32_t crank = paired ? cluster_ctarank() : 0u;
-  const int unit0 = paired ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int unit_stride = paired ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-  const int num_tiles = (paired ? (tiles_m + 1) / 2 : tiles_m) * tiles_n;  // number of work units
-  auto unit_m0 = [&](int u) { return ((paired ? 2 * (u / tiles_n) + (int)crank : u / tiles_n)) * GEMM_BM; };
+  const int num_tiles = tiles_m * tiles_n;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == GEMM_CONSUMERS) {
     tma_prefetch_desc(&p.tm_a_hi);
     tma_prefetch_desc(&p.tm_b_hi);
     if (p.split) {
@@ -361,231 +312,166 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
       tma_prefetch_desc(&p.tm_a_hi8);
       tma_prefetch_desc(&p.tm_b_hi8);
     }
-  }
-  if (warp == 1 && lane == 0) {
     for (int s = 0; s < p.n_stages; ++s) {
-      mbar_init(&full_bar[s], 1);            // cta_group::2: the leader's barrier collects the bytes of both CTAs' loads
-      mbar_init(&empty_bar[s], mc ? 2 : 1);  // mcast: both CTAs' MMAs must have drained the slot
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], tc ? 2 * GEMM_EPI_WARPS : GEMM_EPI_WARPS);  // one arrive per epilogue warp (of both CTAs)
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], GEMM_CONSUMERS / 32);  // one arrive per consumer warp once its wgmma reads of the slot retired
     }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    if constexpr (TWO_CTA) tmem_alloc_2cta<GEMM_TMEM_COLS>(tmem_ptr_smem); else tmem_alloc<GEMM_TMEM_COLS>(tmem_ptr_smem);
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  if (paired) cluster_sync_all();  // the peer's barriers are initialised before anything can arrive on them
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
-  if (warp == 0) {
+  if (warp == GEMM_CONSUMERS / 32) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = unit0; tile < num_tiles; tile += unit_stride) {
-        const int m0 = unit_m0(tile);
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int m0 = (tile / tiles_n) * GEMM_BM;
         const int n0 = (tile % tiles_n) * BN;
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* st = stages + (size_t)stage * stage_bytes;
           const int k0 = kb * GEMM_BK;
           uint8_t* sb = st + GEMM_A_TILE_BYTES * n_parts;
-          if constexpr (TWO_CTA) {
-            // cta_group::2: every load of both CTAs completes on the leader's full barrier
-            const uint32_t lead_full = mapa_cluster(&full_bar[stage], 0);
-            // (the peer never arrives: it cannot load into a slot before the leader's MMA released it, so its bytes always
-            //  belong to the phase the leader arms here)
-            if (crank == 0) mbar_arrive_expect_tx(&full_bar[stage], 2u * (uint32_t)stage_bytes);
-            const int brow2 = n0 + (int)crank * (BN / 2);
-            tma_load_2d_2cta(st, &p.tm_a_hi, lead_full, k0, m0);
-            tma_load_2d_2cta(sb, &p.tm_b_hi, lead_full, k0, brow2);
-            if (p.split == 1) {
-              tma_load_2d_2cta(st + GEMM_A_TILE_BYTES, &p.tm_a_lo, lead_full, k0, m0);
-              tma_load_2d_2cta(sb + b_tile_bytes, &p.tm_b_lo, lead_full, k0, brow2);
-            } else if (p.split == 2) {
-              tma_load_2d_2cta(st + GEMM_A_TILE_BYTES, &p.tm_a_lo, lead_full, k0, m0);
-              tma_load_2d_2cta(st + GEMM_A_TILE_BYTES + GEMM_A_TILE_BYTES / 2, &p.tm_a_hi8, lead_full, k0, m0);
-              tma_load_2d_2cta(sb + b_tile_bytes, &p.tm_b_hi8, lead_full, k0, brow2);
-              tma_load_2d_2cta(sb + b_tile_bytes + b_tile_bytes / 2, &p.tm_b_lo, lead_full, k0, brow2);
-            }
-            if (++stage == p.n_stages) { stage = 0; phase ^= 1; }
-            continue;
-          }
           mbar_arrive_expect_tx(&full_bar[stage], (uint32_t)stage_bytes);
-          // B: whole tile, or (mcast) this CTA's half of the rows, multicast to both CTAs of the pair
-          const int bh = mc ? BN / 2 : 0;  // rows per half
-          const int brow = n0 + (int)crank * bh;
-          auto load_b = [&](uint8_t* dst_tile, int row_bytes, const CUtensorMap* tm) {
-            if (mc) tma_load_2d_mcast(dst_tile + (size_t)crank * bh * row_bytes, tm, &full_bar[stage], k0, brow, (uint16_t)3);
-            else tma_load_2d(dst_tile, tm, &full_bar[stage], k0, n0);
-          };
           tma_load_2d(st, &p.tm_a_hi, &full_bar[stage], k0, m0);
-          load_b(sb, 128, &p.tm_b_hi);
+          tma_load_2d(sb, &p.tm_b_hi, &full_bar[stage], k0, n0);
           if (p.split == 1) {
             tma_load_2d(st + GEMM_A_TILE_BYTES, &p.tm_a_lo, &full_bar[stage], k0, m0);
-            load_b(sb + b_tile_bytes, 128, &p.tm_b_lo);
+            tma_load_2d(sb + b_tile_bytes, &p.tm_b_lo, &full_bar[stage], k0, n0);
           } else if (p.split == 2) {  // [A_lo8 | A_hi8] and [B_hi8 | B_lo8]: 64-byte rows, half the fp16 tile each
             tma_load_2d(st + GEMM_A_TILE_BYTES, &p.tm_a_lo, &full_bar[stage], k0, m0);
             tma_load_2d(st + GEMM_A_TILE_BYTES + GEMM_A_TILE_BYTES / 2, &p.tm_a_hi8, &full_bar[stage], k0, m0);
-            load_b(sb + b_tile_bytes, 64, &p.tm_b_hi8);
-            load_b(sb + b_tile_bytes + b_tile_bytes / 2, 64, &p.tm_b_lo);
+            tma_load_2d(sb + b_tile_bytes, &p.tm_b_hi8, &full_bar[stage], k0, n0);
+            tma_load_2d(sb + b_tile_bytes + b_tile_bytes / 2, &p.tm_b_lo, &full_bar[stage], k0, n0);
           }
           if (++stage == p.n_stages) { stage = 0; phase ^= 1; }
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (cta_group::2: the leader CTA issues for the pair) =====================
-    if (lane == 0 && !(tc && crank != 0)) {
-      const uint32_t fmt = (p.dtype == DT_BF16) ? 1u : 0u;
-      const uint32_t mma_m = tc ? 2 * GEMM_BM : GEMM_BM;
-      // c_format F32 (bit 4) | a_format [7,10) | b_format [10,13) | K-major A,B | N>>3 [17,23) | M>>4 [24,29)
-      const uint32_t idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(BN >> 3) << 17) | ((mma_m >> 4) << 24);
-      int stage = 0;
-      uint32_t phase = 0;
-      int ab = 0;
-      uint32_t aphase = 0;
-      for (int tile = unit0; tile < num_tiles; tile += unit_stride) {
-        mbar_wait(&tmem_empty[ab], aphase ^ 1);
-        tcgen05_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(ab * 256);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tcgen05_fence_after();
-          const uint32_t a_hi = smem_u32(stages + (size_t)stage * stage_bytes);
-          const uint32_t b_hi = a_hi + GEMM_A_TILE_BYTES * n_parts;
-          const uint64_t da_hi = make_sw128_kmajor_desc(a_hi);
-          const uint64_t db_hi = make_sw128_kmajor_desc(b_hi);
-          if constexpr (TWO_CTA) {
-#pragma unroll
-            for (int k = 0; k < GEMM_BK / 16; ++k) umma_f16_2cta(d_tmem, da_hi + 2 * k, db_hi + 2 * k, idesc, (kb | k) != 0);
-            if (p.split == 1) {
-              const uint64_t da_lo = make_sw128_kmajor_desc(a_hi + GEMM_A_TILE_BYTES);
-              const uint64_t db_lo = make_sw128_kmajor_desc(b_hi + b_tile_bytes);
-#pragma unroll
-              for (int k = 0; k < GEMM_BK / 16; ++k) umma_f16_2cta(d_tmem, da_lo + 2 * k, db_hi + 2 * k, idesc, 1u);
-#pragma unroll
-              for (int k = 0; k < GEMM_BK / 16; ++k) umma_f16_2cta(d_tmem, da_hi + 2 * k, db_lo + 2 * k, idesc, 1u);
-            } else if (p.split == 2) {
-              const uint32_t idesc8 = (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((mma_m >> 4) << 24);
-              const uint64_t da_lo8 = make_sw64_kmajor_desc(a_hi + GEMM_A_TILE_BYTES);
-              const uint64_t da_hi8 = make_sw64_kmajor_desc(a_hi + GEMM_A_TILE_BYTES + GEMM_A_TILE_BYTES / 2);
-              const uint64_t db_hi8 = make_sw64_kmajor_desc(b_hi + b_tile_bytes);
-              const uint64_t db_lo8 = make_sw64_kmajor_desc(b_hi + b_tile_bytes + b_tile_bytes / 2);
-#pragma unroll
-              for (int k = 0; k < GEMM_BK / 32; ++k) umma_f8_2cta(d_tmem, da_lo8 + 2 * k, db_hi8 + 2 * k, idesc8, 1u);
-#pragma unroll
-              for (int k = 0; k < GEMM_BK / 32; ++k) umma_f8_2cta(d_tmem, da_hi8 + 2 * k, db_lo8 + 2 * k, idesc8, 1u);
-            }
-            umma_commit_2cta_mcast(&empty_bar[stage], (uint16_t)3);  // frees the slot in both CTAs
-            if (++stage == p.n_stages) { stage = 0; phase ^= 1; }
-            continue;
-          }
-#pragma unroll
-          for (int k = 0; k < GEMM_BK / 16; ++k)  // +32 B per K=16 step inside the 128 B swizzle row
-            umma_f16(d_tmem, da_hi + 2 * k, db_hi + 2 * k, idesc, (kb | k) != 0);
-          if (p.split == 1) {
-            const uint64_t da_lo = make_sw128_kmajor_desc(a_hi + GEMM_A_TILE_BYTES);
-            const uint64_t db_lo = make_sw128_kmajor_desc(b_hi + b_tile_bytes);
-#pragma unroll
-            for (int k = 0; k < GEMM_BK / 16; ++k) umma_f16(d_tmem, da_lo + 2 * k, db_hi + 2 * k, idesc, 1u);
-#pragma unroll
-            for (int k = 0; k < GEMM_BK / 16; ++k) umma_f16(d_tmem, da_hi + 2 * k, db_lo + 2 * k, idesc, 1u);
-          } else if (p.split == 2) {
-            // cross terms at the fp8 rate: A_lo8 * B_hi8 and A_hi8 * B_lo8 (e4m3, K = 32 per instruction)
-            const uint32_t idesc8 = (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(GEMM_BM >> 4) << 24);
-            const uint64_t da_lo8 = make_sw64_kmajor_desc(a_hi + GEMM_A_TILE_BYTES);
-            const uint64_t da_hi8 = make_sw64_kmajor_desc(a_hi + GEMM_A_TILE_BYTES + GEMM_A_TILE_BYTES / 2);
-            const uint64_t db_hi8 = make_sw64_kmajor_desc(b_hi + b_tile_bytes);
-            const uint64_t db_lo8 = make_sw64_kmajor_desc(b_hi + b_tile_bytes + b_tile_bytes / 2);
-#pragma unroll
-            for (int k = 0; k < GEMM_BK / 32; ++k) umma_f8(d_tmem, da_lo8 + 2 * k, db_hi8 + 2 * k, idesc8, 1u);
-#pragma unroll
-            for (int k = 0; k < GEMM_BK / 32; ++k) umma_f8(d_tmem, da_hi8 + 2 * k, db_lo8 + 2 * k, idesc8, 1u);
-          }
-          // frees the smem slot when these MMAs retire (in both CTAs of the pair when the slot is multicast-fed)
-          if (mc) umma_commit_mcast(&empty_bar[stage], (uint16_t)3); else umma_commit(&empty_bar[stage]);
-          if (++stage == p.n_stages) { stage = 0; phase ^= 1; }
-        }
-        if constexpr (TWO_CTA) umma_commit_2cta_mcast(&tmem_full[ab], (uint16_t)3);  // both CTAs' epilogues
-        else umma_commit(&tmem_full[ab]);                                            // accumulator complete -> epilogue
-        if (++ab == 2) { ab = 0; aphase ^= 1; }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================== epilogue =====================
-    const int we = warp & 3;           // TMEM lane quadrant this warp may read
-    const int ehalf = (warp - 4) >> 2;  // which of the two warps of the quadrant
-    float* st = staging + (warp - 4) * (32 * 16);
-    const int et = threadIdx.x - 128;  // 0..255
-    const bool glu = E::GENERIC ? (p.glu != 0) : E::GLU;
-    const int n_out = glu ? p.N / 2 : p.N;
-    const int bn_out = glu ? BN / 2 : BN;
-    int ab = 0;
-    uint32_t aphase = 0;
-    const bool has_mul = E::GENERIC ? (p.mul != nullptr) : E::MUL;
-    const bool has_res = E::GENERIC ? (p.residual != nullptr) : E::RES;
-    // Pull a tile's multiplier / residual rows into L2 one tile ahead of its epilogue, so the epilogue's 128-bit
-    // loads are L2 hits instead of ~1 us DRAM round trips (they cannot be issued deep enough from registers).
-    auto prefetch_tile = [&](int t) {
-      if (!p.epi_prefetch || !(has_mul || has_res) || t >= num_tiles) return;
-      if (et >= GEMM_BM) return;
-      const int row = unit_m0(t) + et;
-      if (row >= p.M) return;
-      const int c0 = (t % tiles_n) * bn_out;
-      for (int c = 0; c < bn_out && c0 + c < n_out; c += 32) {
-        if (has_mul) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.mul + (size_t)row * p.ld_mul + c0 + c));
-        if (has_res) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.residual + (size_t)row * p.ld_res + c0 + c));
-      }
-    };
-    prefetch_tile(unit0);
-    for (int tile = unit0; tile < num_tiles; tile += unit_stride) {
-      prefetch_tile(tile + unit_stride);
-      const int m0 = unit_m0(tile);
-      const int tn = tile % tiles_n;
-      const int n0 = tn * BN;
-      float* sb = sbias + ab * (GEMM_COLVEC_PLANES * 256);
-      // per-column vectors of this tile -> smem (visible to the epilogue warps after the named barrier)
-      for (int c = et; c < BN; c += 32 * GEMM_EPI_WARPS) {
-        sb[c] = (p.bias != nullptr && n0 + c < p.N) ? __ldg(p.bias + n0 + c) : 0.f;
-        if (E::GENERIC ? (p.row_stats != nullptr) : E::LNA) sb[256 + c] = (n0 + c < p.N) ? __ldg(p.ln_c1 + n0 + c) : 0.f;
-        if (E::GENERIC ? (p.res_stats != nullptr) : E::LNR) {
-          const int oc = tn * bn_out + c;  // output column (no GLU with a LayerNorm'd residual)
-          const bool okc = c < bn_out && oc < n_out;
-          sb[512 + c] = okc ? __ldg(p.res_gamma + oc) : 0.f;
-          sb[768 + c] = okc ? __ldg(p.res_beta + oc) : 0.f;
-        }
-      }
-      named_bar_sync(1, 32 * GEMM_EPI_WARPS);
-      const uint32_t t_row = tmem_base + ((uint32_t)(we * 32) << 16) + (uint32_t)(ab * 256);
-      epilogue_tile<E>(p, t_row, sb, st, lane, ehalf, m0 + we * 32, tn, bn_out, n_out, &tmem_full[ab], aphase);  // waits for the accumulator
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (tc && crank != 0) mbar_arrive_cluster(mapa_cluster(&tmem_empty[ab], 0));  // the leader's MMA waits for both CTAs
-        else mbar_arrive(&tmem_empty[ab]);
-      }
-      if (++ab == 2) { ab = 0; aphase ^= 1; }
-    }
+    return;
   }
 
-  tcgen05_fence_before();
-  __syncthreads();
-  if (paired) cluster_sync_all();  // no CTA leaves while its peer may still write into it / arrive on its barriers
-  if (warp == 2) {
-    tcgen05_fence_after();
-    if constexpr (TWO_CTA) tmem_dealloc_2cta<GEMM_TMEM_COLS>(tmem_base); else tmem_dealloc<GEMM_TMEM_COLS>(tmem_base);
+  // ===================== consumers: wgmma main loop + epilogue of rows [64*wg, +64) =====================
+  const int wg = warp >> 2;
+  const int et = threadIdx.x;  // 0..255
+  float* st = staging + warp * (16 * 16);
+  const bool glu = E::GENERIC ? (p.glu != 0) : E::GLU;
+  const int n_out = glu ? p.N / 2 : p.N;
+  const int bn_out = glu ? BN / 2 : BN;
+  const int nch = (BN + 63) / 64;  // 64-column accumulator chunks in use (a chunk past BN reads rows beyond the B tile: discarded)
+  const bool has_mul = E::GENERIC ? (p.mul != nullptr) : E::MUL;
+  const bool has_res = E::GENERIC ? (p.residual != nullptr) : E::RES;
+  // Pull a tile's multiplier / residual rows into L2 one tile ahead of its epilogue, so the epilogue's 128-bit
+  // loads are L2 hits instead of DRAM round trips.
+  auto prefetch_tile = [&](int t) {
+    if (!p.epi_prefetch || !(has_mul || has_res) || t >= num_tiles) return;
+    if (et >= GEMM_BM) return;
+    const int row = (t / tiles_n) * GEMM_BM + et;
+    if (row >= p.M) return;
+    const int c0 = (t % tiles_n) * bn_out;
+    for (int c = 0; c < bn_out && c0 + c < n_out; c += 32) {
+      if (has_mul) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.mul + (size_t)row * p.ld_mul + c0 + c));
+      if (has_res) asm volatile("prefetch.global.L2 [%0];" ::"l"(p.residual + (size_t)row * p.ld_res + c0 + c));
+    }
+  };
+  prefetch_tile(blockIdx.x);
+  int stage = 0;
+  uint32_t phase = 0;
+  int ab = 0;
+  const uint32_t a_off = (uint32_t)wg * 64 * 128;  // this warpgroup's 64 rows of the 128-byte-row A tile
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    prefetch_tile(tile + gridDim.x);
+    const int m0 = (tile / tiles_n) * GEMM_BM;
+    const int tn = tile % tiles_n;
+    const int n0 = tn * BN;
+    // the e4m3 cross terms get an accumulator of their own: fp8 wgmma adds its products into the accumulator with ~14 bits
+    // kept, which would truncate these 2^-11-sized terms against the fp16 sum; their own sum is added in fp32 after the tile
+    float acc[GEMM_MAX_BN / 64][32], acc8[GEMM_MAX_BN / 64][32];
+#pragma unroll
+    for (int c = 0; c < GEMM_MAX_BN / 64; ++c)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) acc[c][i] = acc8[c][i] = 0.f;
+    int prev_stage = -1;
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t a_hi = smem_u32(stages + (size_t)stage * stage_bytes);
+      const uint32_t b_hi = a_hi + GEMM_A_TILE_BYTES * n_parts;
+      const uint64_t da_hi = wgmma_desc_sw128(a_hi + a_off);
+      const uint64_t db_hi = wgmma_desc_sw128(b_hi);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < GEMM_BK / 16; ++k)  // +32 B per K=16 step inside the 128 B swizzle row; +8 KB per 64 B rows
+#pragma unroll
+        for (int c = 0; c < 4; ++c)
+          if (c < nch) wgmma_m64n64k16_ss<E::DT>(acc[c], da_hi + 2 * k, db_hi + 512 * c + 2 * k, 1u);
+      if (p.split == 1) {
+        const uint64_t da_lo = wgmma_desc_sw128(a_hi + GEMM_A_TILE_BYTES + a_off);
+        const uint64_t db_lo = wgmma_desc_sw128(b_hi + b_tile_bytes);
+#pragma unroll
+        for (int k = 0; k < GEMM_BK / 16; ++k)
+#pragma unroll
+          for (int c = 0; c < GEMM_MAX_BN / 64; ++c)
+            if (c < nch) {
+              wgmma_m64n64k16_ss<E::DT>(acc[c], da_lo + 2 * k, db_hi + 512 * c + 2 * k, 1u);
+              wgmma_m64n64k16_ss<E::DT>(acc[c], da_hi + 2 * k, db_lo + 512 * c + 2 * k, 1u);
+            }
+      } else if (p.split == 2) {
+        // cross terms at the fp8 rate: A_lo8 * B_hi8 and A_hi8 * B_lo8 (e4m3, K = 32 per instruction, 64-byte rows)
+        const uint64_t da_lo8 = wgmma_desc_sw64(a_hi + GEMM_A_TILE_BYTES + a_off / 2);
+        const uint64_t da_hi8 = wgmma_desc_sw64(a_hi + GEMM_A_TILE_BYTES + GEMM_A_TILE_BYTES / 2 + a_off / 2);
+        const uint64_t db_hi8 = wgmma_desc_sw64(b_hi + b_tile_bytes);
+        const uint64_t db_lo8 = wgmma_desc_sw64(b_hi + b_tile_bytes + b_tile_bytes / 2);
+#pragma unroll
+        for (int k = 0; k < GEMM_BK / 32; ++k)
+#pragma unroll
+          for (int c = 0; c < GEMM_MAX_BN / 64; ++c)
+            if (c < nch) {
+              wgmma_m64n64k32_e4m3_ss(acc8[c], da_lo8 + 2 * k, db_hi8 + 256 * c + 2 * k);
+              wgmma_m64n64k32_e4m3_ss(acc8[c], da_hi8 + 2 * k, db_lo8 + 256 * c + 2 * k);
+            }
+      }
+      wgmma_commit();
+      // keep this k block in flight; the previous one has retired -> its smem slot goes back to the producer
+      wgmma_wait<1>();
+      if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+      prev_stage = stage;
+      if (++stage == p.n_stages) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+#pragma unroll
+    for (int c = 0; c < GEMM_MAX_BN / 64; ++c) {
+      wgmma_fence_acc(acc[c]);
+      wgmma_fence_acc(acc8[c]);
+    }
+    if (p.split == 2) {
+#pragma unroll
+      for (int c = 0; c < GEMM_MAX_BN / 64; ++c)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) acc[c][i] += acc8[c][i];
+    }
+    if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+    // per-column vectors of this tile -> smem (double-buffered: the other buffer may still be read by the slower warpgroup)
+    float* sb = sbias + ab * (GEMM_COLVEC_PLANES * 256);
+    for (int c = et; c < BN; c += GEMM_CONSUMERS) {
+      sb[c] = (p.bias != nullptr && n0 + c < p.N) ? __ldg(p.bias + n0 + c) : 0.f;
+      if (E::GENERIC ? (p.row_stats != nullptr) : E::LNA) sb[256 + c] = (n0 + c < p.N) ? __ldg(p.ln_c1 + n0 + c) : 0.f;
+      if (E::GENERIC ? (p.res_stats != nullptr) : E::LNR) {
+        const int oc = tn * bn_out + c;  // output column (no GLU with a LayerNorm'd residual)
+        const bool okc = c < bn_out && oc < n_out;
+        sb[512 + c] = okc ? __ldg(p.res_gamma + oc) : 0.f;
+        sb[768 + c] = okc ? __ldg(p.res_beta + oc) : 0.f;
+      }
+    }
+    named_bar_sync(1, GEMM_CONSUMERS);
+    epilogue_tile<E>(p, acc, sb, st, lane, m0 + wg * 64 + (warp & 3) * 16, tn, bn_out, n_out);
+    ab ^= 1;
   }
 }
 
-inline size_t gemm_smem_bytes(int block_n, int split, int n_stages, int two_cta = 0) {
-  const size_t stage = (size_t)(GEMM_A_TILE_BYTES + (two_cta ? block_n / 2 : block_n) * 128) * (split ? 2 : 1);
-  return 1024 /*align slack*/ + n_stages * stage + GEMM_STAGING_BYTES + 2 * GEMM_COLVEC_PLANES * 256 * 4 + (2 * GEMM_MAX_STAGES + 4) * 8 + 16;
+inline size_t gemm_smem_bytes(int block_n, int split, int n_stages) {
+  const size_t stage = (size_t)(GEMM_A_TILE_BYTES + block_n * 128) * (split ? 2 : 1);
+  return 1024 /*align slack*/ + n_stages * stage + GEMM_STAGING_BYTES + 2 * GEMM_COLVEC_PLANES * 256 * 4 + 2 * GEMM_MAX_STAGES * 8 + 16;
 }
 
 }  // namespace vima

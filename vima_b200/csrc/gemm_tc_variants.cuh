@@ -33,37 +33,17 @@ cudaError_t launch_gemm_tc_dt(const GemmParams& p, const GemmLaunch& l, int grid
 cudaError_t launch_gemm_tc_f16(const GemmParams& p, const GemmLaunch& l, int grid, size_t smem, int max_smem, cudaStream_t stream);
 cudaError_t launch_gemm_tc_bf16(const GemmParams& p, const GemmLaunch& l, int grid, size_t smem, int max_smem, cudaStream_t stream);
 
-template <class E, bool TWO_CTA>
-inline cudaError_t launch_kernel(const GemmParams& p, int grid, size_t smem, int max_smem, cudaStream_t stream, int device) {
+template <class E>
+inline cudaError_t launch_one(const GemmParams& p, int grid, size_t smem, int max_smem, cudaStream_t stream, int device) {
   static bool attr_set[64] = {};  // per instantiation and device (function attributes are per device)
   const int di = device & 63;
   if (!attr_set[di]) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<E, TWO_CTA>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);
+    cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<E>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);
     if (e != cudaSuccess) return e;
     attr_set[di] = true;
   }
-  if (p.mcast || TWO_CTA) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(GEMM_THREADS);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, gemm_tc_kernel<E, TWO_CTA>, p);
-  }
-  gemm_tc_kernel<E, TWO_CTA><<<grid, GEMM_THREADS, smem, stream>>>(p);
+  gemm_tc_kernel<E><<<grid, GEMM_THREADS, smem, stream>>>(p);
   return cudaGetLastError();
-}
-
-template <class E>
-inline cudaError_t launch_one(const GemmParams& p, int grid, size_t smem, int max_smem, cudaStream_t stream, int device) {
-  return p.two_cta ? launch_kernel<E, true>(p, grid, smem, max_smem, stream, device) : launch_kernel<E, false>(p, grid, smem, max_smem, stream, device);
 }
 
 template <int DT>

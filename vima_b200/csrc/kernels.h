@@ -40,10 +40,10 @@ constexpr int ATTN_TAIL_MAX_ROWS = 8;          // attention_tail.cu: query rows 
 cudaError_t launch_attention(const AttnParams& p, cudaStream_t stream);
 size_t attention_smem_bytes(const AttnParams& p);             // dynamic shared memory the mma.sync kernel needs for p
 int attention_max_lk(const AttnParams& p, size_t smem_limit);  // largest Lk (multiple of 64) that fits smem_limit at p's format
-bool attention_tc_supported(const AttnParams& p);  // tcgen05 variant (attention_tc.cu): head_dim 32, split operands, no bias, Lk <= 512
+bool attention_tc_supported(const AttnParams& p);  // wgmma variant (attention_tc.cu): head_dim 32, split operands, no bias, Lk <= 512
 cudaError_t launch_attention_tc(const AttnParams& p, void* encode_tiled_fn, cudaStream_t stream);  // encode_tiled_fn: cuTensorMapEncodeTiled
 // query rows [row0, row0 + nt) of every (batch, head) (nt <= ATTN_TAIL_MAX_ROWS, head_dim 32, Lk <= 512): the rows that would
-// otherwise occupy a nearly empty 128-row tile of the tcgen05 kernel
+// otherwise occupy a nearly empty 128-row tile of the wgmma kernel
 cudaError_t launch_attention_tail(const AttnParams& p, int row0, int nt, cudaStream_t stream);
 
 struct SmallAttnParams {  // tiny-sequence fp32 attention (ViT: 5 tokens, 24 heads of 32)

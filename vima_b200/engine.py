@@ -52,7 +52,7 @@ def prec() -> Prec:
 def ctx_for(t: torch.Tensor) -> _C.Context:
     if not t.is_cuda:
         raise RuntimeError(
-            "vima_b200 modules only run on a CUDA (sm_100a) device: got a CPU tensor. There is no CPU / eager fallback."
+            "vima_b200 modules only run on a CUDA (sm_90a) device: got a CPU tensor. There is no CPU / eager fallback."
         )
     return _C.Context.get(t.device)
 

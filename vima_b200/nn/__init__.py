@@ -1,4 +1,4 @@
-"""`vima.nn` surface (reference: /root/reference/vima/nn/__init__.py:1-6) on sm_100a kernels."""
+"""`vima.nn` surface (reference: /root/reference/vima/nn/__init__.py:1-6) on sm_90a kernels."""
 from .action import (
     ActionDecoder,
     ActionEmbedding,

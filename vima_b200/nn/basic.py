@@ -58,12 +58,12 @@ class F32GroupRunner:
 
 
 def _use_tensor_cores(in_features: int, rows: int) -> bool:
-    # tcgen05 path needs K % 8 == 0 (TMA row pitch); tiny-K layers run exact fp32 on CUDA cores
+    # wgmma path needs K % 8 == 0 (TMA row pitch); tiny-K layers run exact fp32 on CUDA cores
     return in_features % 8 == 0 and in_features >= 64
 
 
 class Linear(nn.Linear):
-    """nn.Linear with the reference's parameters whose forward is the tcgen05 GEMM (or exact fp32 for tiny K)."""
+    """nn.Linear with the reference's parameters whose forward is the wgmma GEMM (or exact fp32 for tiny K)."""
 
     def __init__(self, *a, **k):
         super().__init__(*a, **k)

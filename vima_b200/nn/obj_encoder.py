@@ -4,10 +4,10 @@ Module surface / state-dict keys of /root/reference/vima/nn/obj_encoder/obj_enco
 vit/vit.py:13-46,137-236; preprocessing of vit/preprocess.py:9-43.  Kernel plan per call (both views share the ViT,
 so their crops are batched through it together):
 
-    patchify (uint8 -> normalised patch rows, fused /255, -mean, /std)  -> conv1 as tcgen05 GEMM -> +cls +pos
+    patchify (uint8 -> normalised patch rows, fused /255, -mean, /std)  -> conv1 as wgmma GEMM -> +cls +pos
     -> ln_pre [+ ln_1 chained] -> 4 x { in_proj GEMM (+bias) -> 5-token fp32 attention -> out_proj GEMM (+bias
     +residual) -> ln_2 -> c_fc GEMM (+bias, QuickGELU) -> c_proj GEMM (+bias +residual) -> next ln_1 } -> ln_post on
-    the CLS rows -> projection GEMM;   bbox: /[256,128,128,256] -> fp32 K=4 layer -> two tcgen05 GEMMs;
+    the CLS rows -> projection GEMM;   bbox: /[256,128,128,256] -> fp32 K=4 layer -> two wgmma GEMMs;
     per view Linear(1536 -> E) over the [vit | bbox] operand written in place by the two producers.
 """
 from __future__ import annotations

@@ -3,7 +3,7 @@
 
 Parameter tree and state-dict keys are those of HF's PerceiverModel (`model.embeddings.latents`,
 `model.encoder.cross_attention.*`, `model.encoder.self_attends.N.*`); the arithmetic -- LayerNorms, the q / k|v / output /
-MLP projections (tcgen05 GEMMs with GELU and residual epilogues) and the latent attention -- runs on the sm_100a kernels.
+MLP projections (wgmma GEMMs with GELU and residual epilogues) and the latent attention -- runs on the sm_90a kernels.
 """
 from __future__ import annotations
 

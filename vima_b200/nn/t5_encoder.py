@@ -5,7 +5,7 @@ T5 encoder :61-825) and word_embd.py:8-23, without depending on `transformers`: 
 12 heads x 64, d_ff 3072 ReLU, bias-free Linears, UNSCALED dot-product scores plus a shared relative-position bias
 (32 buckets, max distance 128, bidirectional) with the key mask folded in (prompt_encoder.py:785-797).
 
-Kernel plan: RMSNorm (warp-shuffle) -> fused [q;k;v] tcgen05 GEMM -> fused attention (bias looked up from a
+Kernel plan: RMSNorm (warp-shuffle) -> fused [q;k;v] wgmma GEMM -> fused attention (bias looked up from a
 [heads, 2*Lp-1] table in shared memory; the reference materialises a B*H*Lp*Lp tensor) -> o GEMM (+residual) ->
 RMSNorm -> wi GEMM (ReLU epilogue) -> wo GEMM (+residual) -> ... -> final RMSNorm.
 """

@@ -1,7 +1,7 @@
 """XAttnGPT: cross-attention to the prompt alternating with causal self-attention over the obs/action history.
 
 Module surface and state-dict keys of /root/reference/vima/nn/seq_modeling/xattn_gpt/{xattn_gpt.py:13-177,
-components.py:14-263}; the arithmetic runs on the sm_100a kernels (tcgen05 GEMMs with fused bias / GELU / GEGLU /
+components.py:14-263}; the arithmetic runs on the sm_90a kernels (wgmma GEMMs with fused bias / GELU / GEGLU /
 residual epilogues, fused masked attention, warp-shuffle LayerNorm).  Per layer (reference order, xattn_gpt.py:123-132):
 
     XAttention (pre-LN, bias-free, components.py:158-228)        Block (GPT-1 post-LN, components.py:23-37)

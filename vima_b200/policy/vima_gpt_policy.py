@@ -3,7 +3,7 @@
 
 Same causal sequence as VIMA-Gato, [encoded prompt | separator | o0 a0 o1 a1 ...], through `HFGPT`; the image encoder is
 the CLS-token rectangular ViT applied to both views with the two features concatenated (2E wide).  Constructor,
-sub-module names (state-dict keys) and methods follow the reference; the arithmetic runs on the same sm_100a kernels.
+sub-module names (state-dict keys) and methods follow the reference; the arithmetic runs on the same sm_90a kernels.
 """
 from __future__ import annotations
 

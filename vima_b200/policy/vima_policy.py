@@ -1,7 +1,7 @@
 """VIMAPolicy: the drop-in policy class (reference: /root/reference/vima/policy/vima_policy.py:11-322).
 
 Same constructor, sub-module names (state-dict prefixes) and five entry methods as the reference; every tensor op
-between the inputs and the returned tensors runs in the sm_100a kernels of libvima_b200.so.  Host Python only builds
+between the inputs and the returned tensors runs in the sm_90a kernels of libvima_b200.so.  Host Python only builds
 the prompt index map from `token_types` (lists of ints) and launches kernels; there are no per-token Python loops on
 tensors and no host synchronisation after the first call's input checks.
 """
