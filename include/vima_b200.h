@@ -207,8 +207,13 @@ typedef struct {
    * key_mask rows have pitch mask_ld (0 = Lk), and under `causal` query row i sits at key position q_pos0 + i. */
   int kv_batch_rows, mask_ld, q_pos0;
   /* ---- v4 end ---- */
+  /* v5: per-batch causal positions (slot decode: every episode of the batch at its own history length).  DEVICE int [B] or NULL.
+   * When set (causal only, no rel_bias), batch element b has query row i at key position q_pos[b] + i and Lk_b = q_pos[b] + Lq
+   * keys; `Lk` then only bounds the capacity (q_pos[b] in [0, Lk - Lq]) and q_pos0 is ignored. */
+  const int* q_pos;
 } vima_attn_desc;
-#define VIMA_ATTN_DESC_V4_SIZE sizeof(vima_attn_desc)
+#define VIMA_ATTN_DESC_V4_SIZE offsetof(vima_attn_desc, q_pos)
+#define VIMA_ATTN_DESC_V5_SIZE sizeof(vima_attn_desc)
 int vima_attention(vima_ctx*, const vima_attn_desc* d, void* stream);
 
 /* HF modeling_perceiver.py PerceiverSelfAttention (the resampler of vima/nn/obj_encoder/perceiver/perceiver.py:11-41), fp32:
@@ -228,6 +233,25 @@ int vima_assemble_history(vima_ctx*, const float* obs, const uint8_t* obs_mask, 
                           float* tokens, uint8_t* masks_bl, int64_t* pos_bl, void* stream);
 /* pos[b, l] = cumsum(mask[b, :l+1]) - 1   (vima_policy.py:147) */
 int vima_mask_cumsum(vima_ctx*, const uint8_t* mask, int B, int L, int64_t* pos, void* stream);
+
+/* ---- slot decode: every row of the batch is a slot holding one episode at its own history length (DESIGN.md 7 (f)1) ----------
+ * Per-slot DEVICE state, int32 [S] each: len (cache columns used), n_valid (next position id), has_action (0 before the slot's
+ * first step), active.  A step block has Q+1 rows per slot: [action, obs_1..obs_Q] once the slot has an action, else
+ * [obs_1..obs_Q, dummy] with a zero, masked dummy row that no real row sees (causality) and the next step overwrites.
+ * step_begin: obs fp32 [S, Q, E], obs_mask uint8 [S, Q], action fp32 [S, E] -> tokens fp32 [S*(Q+1), E], step_mask uint8 [S, Q+1],
+ * pos int64 [S, Q+1] (n_valid + running count of valid tokens - 1; 0 on inactive slots), q_pos int32 [S] (len, 0 on inactive slots),
+ * and step_mask into columns q_pos .. q_pos+Q of slot_mask uint8 [S, Lmax]. */
+int vima_slot_step_begin(vima_ctx*, const float* obs, const uint8_t* obs_mask, const float* action, int S, int Q, int E, int Lmax,
+                         const int32_t* len, const int32_t* n_valid, const int32_t* has_action, const int32_t* active, float* tokens,
+                         uint8_t* step_mask, int64_t* pos, int32_t* q_pos, uint8_t* slot_mask, void* stream);
+/* Per layer: columns [col0, col0 + width) of the step's rows qkv [S*Lq, ld_qkv] (hi, lo|NULL 16-bit) -> cache rows
+ * b*Lmax + q_pos[b] + r of kv [S*Lmax, ld_kv].  width, col0, ld_* multiples of 8 elements, 16-byte aligned bases. */
+int vima_slot_kv_append(vima_ctx*, const void* qkv_hi, const void* qkv_lo, int ld_qkv, int col0, int width, int S, int Lq, const int32_t* q_pos,
+                        void* kv_hi, void* kv_lo, int ld_kv, int Lmax, void* stream);
+/* out[b] = x[b*(Q+1) + Q-1+has_action[b]] (fp32 rows of E, pitch ldx); then, for active slots, len += Q + has_action,
+ * n_valid += sum(step_mask[b]), has_action = 1. */
+int vima_slot_step_end(vima_ctx*, const float* x, int ldx, int S, int Q, int E, const uint8_t* step_mask, int32_t* len, int32_t* n_valid,
+                       int32_t* has_action, const int32_t* active, float* out, void* stream);
 /* out[b,l,:] = tok[b*stride_b + l*stride_l + :] + table[ids[b,l]]  (xattn_gpt.py:103-105,110-114); out-of-range
  * ids set *err_flag (device int) to 1 -- the reference raises IndexError there. */
 int vima_add_pos_embed(vima_ctx*, const float* tok, int64_t stride_b, int64_t stride_l, const int64_t* ids, const float* table, int n_pos,

@@ -1,0 +1,160 @@
+"""Slot decode vs lockstep decode in a simulated vectorised environment (cfg3 shapes: 200M, 256 slots, Q = 32 obs tokens, Lp = 256).
+
+Episode lengths are drawn from a seeded uniform distribution over 1..--max-steps environment steps (15 * 33 tokens fit the 512
+positions).  Every episode runs to its end in each of three runs, and each run reports completed env-steps/s and episodes/s:
+
+  lockstep  start_decode / forward_step: episodes go in batches of --slots and a batch runs until its longest episode ends
+  eager     open_slots / step_slots: a slot whose episode ended takes the next episode before the next tick (admit), or is released
+  graph     the same schedule with the step replayed from one CUDA graph (capture time reported, not counted)
+
+Admission (the prompt key/value GEMMs of the new episodes) is included in the slot runs' totals and also reported on its own
+(CUDA events).  Weights are random (timing only).  Prints the GPU's name and power limit beside the numbers, one JSON line per run.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import numpy as np
+import torch
+
+import vima_b200
+from oracle import synth  # model shapes only
+
+
+def gpu_info() -> str:
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True, timeout=30)
+        line = r.stdout.strip().splitlines()[torch.cuda.current_device()]
+        return line
+    except Exception:  # noqa: BLE001 -- the name alone is still worth printing
+        return f"{torch.cuda.get_device_name()}, power limit not readable"
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--model", default="200M")
+    ap.add_argument("--slots", type=int, default=256)
+    ap.add_argument("--n-obj", type=int, default=32)
+    ap.add_argument("--prompt-len", type=int, default=256)
+    ap.add_argument("--max-steps", type=int, default=15)
+    ap.add_argument("--episodes", type=int, default=1024)
+    ap.add_argument("--precision", default="f16f8")
+    ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--runs", default="lockstep,eager,graph")
+    a = ap.parse_args()
+    if not torch.cuda.is_available():
+        raise SystemExit("slot_decode_bench needs a CUDA device")
+    vima_b200.set_precision(a.precision)
+    torch.manual_seed(a.seed)
+    pol = vima_b200.VIMAPolicy(**synth.MODEL_CFGS[a.model]).cuda().eval()
+    E, S, Q, Lp = pol.embed_dim, a.slots, a.n_obj, a.prompt_len
+    Lmax = a.max_steps * (Q + 1)
+    lengths = np.random.default_rng(a.seed).integers(1, a.max_steps + 1, size=a.episodes).tolist()
+    total_steps = int(sum(lengths))
+    g = torch.Generator(device="cuda").manual_seed(a.seed)
+    obs_pool = [torch.randn(1, S, Q, E, device="cuda", generator=g) for _ in range(3)]
+    msk = torch.rand(1, S, Q, device="cuda", generator=g) > 0.1
+    msk[..., 0] = True
+    act = torch.randn(1, S, E, device="cuda", generator=g)
+    prompts = torch.randn(Lp, S, E, device="cuda", generator=g)
+    pmask = torch.ones(S, Lp, dtype=torch.bool, device="cuda")
+    info = gpu_info()
+    print(f"# {info}; model {a.model}, {S} slots, Q={Q}, Lp={Lp}, {a.precision}; {a.episodes} episodes of 1..{a.max_steps} steps "
+          f"({total_steps} env-steps, seed {a.seed})")
+
+    def lockstep():
+        ticks = 0
+        for i in range(0, len(lengths), S):
+            batch = lengths[i:i + S]
+            n = len(batch)
+            cache = pol.start_decode(prompts[:, :n], pmask[:n], max_tokens=Lmax)
+            for t in range(max(batch)):
+                pol.forward_step(cache, obs_pool[t % 3][:, :n], msk[:, :n], None if t == 0 else act[:, :n])
+                ticks += 1
+        return ticks, 0.0
+
+    def slotted(step, cache):
+        """Runs every episode through `cache`; returns (ticks, admission ms)."""
+        queue = list(range(len(lengths)))
+        remaining = [0] * S
+        adm_ms, ticks = [], 0
+        pending = list(range(S))  # free slots waiting for an episode
+        while True:
+            take = pending[:len(queue)]
+            if take:
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+                pol.admit(cache, take, prompts[:, :len(take)], pmask[:len(take)])
+                e1.record()
+                adm_ms.append((e0, e1))
+                for b in take:
+                    remaining[b] = lengths[queue.pop(0)]
+            idle = pending[len(take):]
+            if idle:
+                pol.release(cache, idle)
+            if not any(remaining):
+                break
+            step(cache, obs_pool[ticks % 3], msk, act)
+            ticks += 1
+            pending = []
+            for b in range(S):
+                if remaining[b]:
+                    remaining[b] -= 1
+                    if remaining[b] == 0:
+                        pending.append(b)
+        torch.cuda.synchronize()
+        return ticks, sum(e0.elapsed_time(e1) for e0, e1 in adm_ms)
+
+    runs = a.runs.split(",")
+    results = []
+    with torch.no_grad():
+        # warm-up: modules, weight packing, kernel attributes
+        c = pol.open_slots(S, max_tokens=Lmax, max_prompt_tokens=Lp)
+        pol.admit(c, list(range(S)), prompts, pmask)
+        for _ in range(2):
+            pol.step_slots(c, obs_pool[0], msk, act)
+        cd = pol.start_decode(prompts, pmask, max_tokens=Lmax)
+        for t in range(2):
+            pol.forward_step(cd, obs_pool[0], msk, None if t == 0 else act)
+        del c, cd
+        torch.cuda.synchronize()
+        for name in runs:
+            extra = {}
+            if name == "lockstep":
+                fn = lockstep
+            elif name == "eager":
+                cache = pol.open_slots(S, max_tokens=Lmax, max_prompt_tokens=Lp)
+                fn = lambda: slotted(pol.step_slots, cache)  # noqa: E731
+            elif name == "graph":
+                cache = pol.open_slots(S, max_tokens=Lmax, max_prompt_tokens=Lp)
+                pol.admit(cache, list(range(S)), prompts, pmask)
+                t0 = time.perf_counter()
+                gs = pol.capture_step_slots(cache, obs_pool[0], msk, act)
+                torch.cuda.synchronize()
+                extra = {"capture_s": round(time.perf_counter() - t0, 3), "vima_kernels_per_replay": gs.kernels_per_replay}
+                pol.release(cache, list(range(S)))
+                fn = lambda: slotted(lambda c, o, m, x: gs(o, m, x), cache)  # noqa: E731
+            else:
+                raise SystemExit(f"unknown run {name}")
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            ticks, adm = fn()
+            torch.cuda.synchronize()
+            dt = time.perf_counter() - t0
+            r = {"run": name, "seconds": round(dt, 4), "ticks": ticks, "env_steps_per_s": round(total_steps / dt, 1),
+                 "episodes_per_s": round(len(lengths) / dt, 2), "ms_per_tick": round(dt * 1e3 / ticks, 3)}
+            if name != "lockstep":
+                r["admission_ms_total"] = round(adm, 2)
+                r["admission_ms_per_episode"] = round(adm / len(lengths), 4)
+            r.update(extra)
+            r["gpu"] = info
+            results.append(r)
+            print(json.dumps(r), flush=True)
+
+
+if __name__ == "__main__":
+    main()

@@ -82,6 +82,8 @@ class AttnDesc(C.Structure):
         ("scale", c_float), ("causal", c_int), ("dtype", c_int),
         ("o_lo8", c_void_p), ("o_hi8", c_void_p), ("ldo8", c_int),
         ("kv_batch_rows", c_int), ("mask_ld", c_int), ("q_pos0", c_int),
+        # v5
+        ("q_pos", c_void_p),
     ]
 
 
@@ -93,6 +95,7 @@ EXPORTS = [
     "vima_attention", "vima_small_attention", "vima_assemble_history", "vima_mask_cumsum", "vima_add_pos_embed",
     "vima_gather_prompt", "vima_patchify", "vima_vit_tokens", "vima_bbox_norm", "vima_fill_ee", "vima_max_u8",
     "vima_action_scale", "vima_action_postprocess", "vima_latent_attention", "vima_object_stats", "vima_crop_resize", "vima_head_select", "vima_gato_positions", "vima_pack_weight_f8", "vima_split_f8",
+    "vima_slot_step_begin", "vima_slot_kv_append", "vima_slot_step_end",
 ]
 
 
@@ -268,8 +271,9 @@ class Context:
         self._ck(self.lib.vima_norm(self.h, C.byref(d), c_void_p(self._s())), "norm")
 
     def attention(self, *, q, k, v, o, B, H, Lq, Lk, D, scale, causal=False, key_mask=None, rel_bias=None, dtype=DT_F16, o8=None,
-                  kv_batch_rows=0, mask_ld=0, q_pos0=0):
-        """q, k, v, o: (hi, lo|None, ld, column offset) tuples over 16-bit operand buffers."""
+                  kv_batch_rows=0, mask_ld=0, q_pos0=0, q_pos=None):
+        """q, k, v, o: (hi, lo|None, ld, column offset) tuples over 16-bit operand buffers.  q_pos: int32 [B] on the device, the
+        causal position of each batch element's first query row (its key count is then q_pos[b] + Lq; Lk is the capacity)."""
         es = 2
 
         def at(t, off):
@@ -285,6 +289,9 @@ class Context:
         d.B, d.H, d.Lq, d.Lk, d.D = int(B), int(H), int(Lq), int(Lk), int(D)
         d.scale, d.causal, d.dtype = float(scale), int(causal), dtype
         d.kv_batch_rows, d.mask_ld, d.q_pos0 = int(kv_batch_rows), int(mask_ld), int(q_pos0)
+        if q_pos is not None:
+            assert q_pos.dtype == torch.int32 and q_pos.is_contiguous() and q_pos.numel() >= B
+            d.q_pos = q_pos.data_ptr()
         if o8 is not None:  # (lo8, hi8) uint8 [rows, ld8]
             d.o_lo8, d.o_hi8, d.ldo8 = o8[0].data_ptr(), o8[1].data_ptr(), o8[0].stride(0)
         self._ck(self.lib.vima_attention(self.h, C.byref(d), c_void_p(self._s())), "attention")
@@ -305,6 +312,28 @@ class Context:
     def mask_cumsum(self, mask_u8, pos):
         B, L = mask_u8.shape
         self._ck(self.lib.vima_mask_cumsum(self.h, c_void_p(mask_u8.data_ptr()), B, L, c_void_p(pos.data_ptr()), c_void_p(self._s())), "mask_cumsum")
+
+    # ---------------------------------------------------------------- slot decode (per-slot int32 state vectors on the device)
+    def slot_step_begin(self, obs, obs_mask_u8, action, *, Lmax, len_, n_valid, has_action, active, tokens, step_mask, pos, q_pos, slot_mask):
+        """obs fp32 [S, Q, E], obs_mask uint8 [S, Q], action fp32 [S, E] -> tokens [S*(Q+1), E], step_mask [S, Q+1], pos int64 [S, Q+1],
+        q_pos int32 [S]; writes the step's columns of slot_mask [S, Lmax]."""
+        S, Q, E = obs.shape
+        self._ck(self.lib.vima_slot_step_begin(self.h, c_void_p(obs.data_ptr()), c_void_p(obs_mask_u8.data_ptr()), c_void_p(action.data_ptr()),
+                                               S, Q, E, int(Lmax), c_void_p(len_.data_ptr()), c_void_p(n_valid.data_ptr()),
+                                               c_void_p(has_action.data_ptr()), c_void_p(active.data_ptr()), c_void_p(tokens.data_ptr()),
+                                               c_void_p(step_mask.data_ptr()), c_void_p(pos.data_ptr()), c_void_p(q_pos.data_ptr()),
+                                               c_void_p(slot_mask.data_ptr()), c_void_p(self._s())), "slot_step_begin")
+
+    def slot_kv_append(self, qkv_hi, qkv_lo, ld_qkv, col0, width, S, Lq, q_pos, kv_hi, kv_lo, ld_kv, Lmax):
+        self._ck(self.lib.vima_slot_kv_append(self.h, c_void_p(qkv_hi.data_ptr()), c_void_p(_ptr(qkv_lo)), int(ld_qkv), int(col0), int(width),
+                                              int(S), int(Lq), c_void_p(q_pos.data_ptr()), c_void_p(kv_hi.data_ptr()), c_void_p(_ptr(kv_lo)),
+                                              int(ld_kv), int(Lmax), c_void_p(self._s())), "slot_kv_append")
+
+    def slot_step_end(self, x, S, Q, E, step_mask, *, len_, n_valid, has_action, active, out):
+        """x fp32 [S*(Q+1), >=E] -> out [S, E] (each slot's prediction row); advances the active slots' state."""
+        self._ck(self.lib.vima_slot_step_end(self.h, c_void_p(x.data_ptr()), x.stride(0), int(S), int(Q), int(E), c_void_p(step_mask.data_ptr()),
+                                             c_void_p(len_.data_ptr()), c_void_p(n_valid.data_ptr()), c_void_p(has_action.data_ptr()),
+                                             c_void_p(active.data_ptr()), c_void_p(out.data_ptr()), c_void_p(self._s())), "slot_step_end")
 
     def add_pos_embed(self, tok, stride_b, stride_l, ids, table, B, L, E, *, out_f32=None, hi=None, lo=None, dtype=DT_F16, err_flag=None):
         self._ck(self.lib.vima_add_pos_embed(self.h, c_void_p(tok.data_ptr()), c_i64(stride_b), c_i64(stride_l), c_void_p(ids.data_ptr()),

@@ -386,8 +386,11 @@ int vima_attention(vima_ctx* c, const vima_attn_desc* d_in, void* stream) {
   p.scale = d->scale; p.causal = d->causal; p.split = split; p.dtype = d->dtype;
   p.o_lo8 = (unsigned char*)d->o_lo8; p.o_hi8 = (unsigned char*)d->o_hi8; p.ldo8 = d->ldo8;
   p.kv_batch_rows = d->kv_batch_rows; p.mask_ld = d->mask_ld; p.q_pos0 = d->q_pos0; p.q_batch_rows = 0;
+  p.q_pos = d->q_pos;
   if ((d->kv_batch_rows && d->kv_batch_rows < d->Lk) || (d->mask_ld && d->mask_ld < d->Lk) || d->q_pos0 < 0)
     return fail(c, VIMA_E_INVALID, "attention: kv_batch_rows / mask_ld must cover Lk, q_pos0 >= 0");
+  if (d->q_pos && (!d->causal || d->rel_bias || d->Lq > d->Lk))
+    return fail(c, VIMA_E_INVALID, "attention: per-batch q_pos needs causal attention, no relative bias and Lq <= Lk");
   if ((p.o_lo8 == nullptr) != (p.o_hi8 == nullptr) || (p.o_lo8 && ((p.ldo8 & 1) || d->dtype != DT_F16)))
     return fail(c, VIMA_E_INVALID, "attention: o_lo8/o_hi8 come together (fp16 format, even ldo8)");
   // wgmma kernel for the shapes it takes (head_dim 32, split operands, no relative bias), mma.sync kernel otherwise;
@@ -456,6 +459,41 @@ int vima_assemble_history(vima_ctx* c, const float* obs, const uint8_t* obs_mask
 int vima_mask_cumsum(vima_ctx* c, const uint8_t* mask, int B, int L, int64_t* pos, void* stream) {
   CHECK_CTX(c);
   LAUNCHED(c, launch_mask_cumsum(mask, B, L, (long long*)pos, (cudaStream_t)stream), "mask_cumsum");
+}
+
+int vima_slot_step_begin(vima_ctx* c, const float* obs, const uint8_t* obs_mask, const float* action, int S, int Q, int E, int Lmax,
+                         const int32_t* len, const int32_t* n_valid, const int32_t* has_action, const int32_t* active, float* tokens,
+                         uint8_t* step_mask, int64_t* pos, int32_t* q_pos, uint8_t* slot_mask, void* stream) {
+  CHECK_CTX(c);
+  if (!obs || !obs_mask || !action || !len || !n_valid || !has_action || !active || !tokens || !step_mask || !pos || !q_pos || !slot_mask)
+    return fail(c, VIMA_E_INVALID, "slot_step_begin: null pointer");
+  if (S < 0 || Q < 1 || (E & 3) || E <= 0 || Q + 1 > Lmax || ((uintptr_t)obs & 15) || ((uintptr_t)action & 15) || ((uintptr_t)tokens & 15))
+    return fail(c, VIMA_E_INVALID, "slot_step_begin: S >= 0, 1 <= Q < Lmax, E %% 4 == 0, 16-byte aligned fp32 rows");
+  LAUNCHED(c, launch_slot_step_begin(obs, obs_mask, action, S, Q, E, Lmax, len, n_valid, has_action, active, tokens, step_mask,
+                                     (long long*)pos, q_pos, slot_mask, (cudaStream_t)stream),
+           "slot_step_begin");
+}
+
+int vima_slot_kv_append(vima_ctx* c, const void* qkv_hi, const void* qkv_lo, int ld_qkv, int col0, int width, int S, int Lq, const int32_t* q_pos,
+                        void* kv_hi, void* kv_lo, int ld_kv, int Lmax, void* stream) {
+  CHECK_CTX(c);
+  if (!qkv_hi || !kv_hi || !q_pos || (qkv_lo == nullptr) != (kv_lo == nullptr)) return fail(c, VIMA_E_INVALID, "slot_kv_append: null pointer");
+  auto al = [](const void* q) { return ((uintptr_t)q & 15) == 0; };
+  if ((ld_qkv & 7) || (col0 & 7) || (width & 7) || (ld_kv & 7) || width <= 0 || col0 + width > ld_qkv || width > ld_kv || Lq < 1 || Lq > Lmax ||
+      !al(qkv_hi) || !al(qkv_lo) || !al(kv_hi) || !al(kv_lo))
+    return fail(c, VIMA_E_INVALID, "slot_kv_append: ld / col0 / width multiples of 8 inside the rows, 16-byte aligned bases, Lq <= Lmax");
+  LAUNCHED(c, launch_slot_kv_append((const unsigned short*)qkv_hi, (const unsigned short*)qkv_lo, ld_qkv, col0, width, S, Lq, q_pos,
+                                    (unsigned short*)kv_hi, (unsigned short*)kv_lo, ld_kv, Lmax, (cudaStream_t)stream),
+           "slot_kv_append");
+}
+
+int vima_slot_step_end(vima_ctx* c, const float* x, int ldx, int S, int Q, int E, const uint8_t* step_mask, int32_t* len, int32_t* n_valid,
+                       int32_t* has_action, const int32_t* active, float* out, void* stream) {
+  CHECK_CTX(c);
+  if (!x || !step_mask || !len || !n_valid || !has_action || !active || !out) return fail(c, VIMA_E_INVALID, "slot_step_end: null pointer");
+  if (S < 0 || Q < 1 || (E & 3) || E <= 0 || (ldx & 3) || ldx < E || ((uintptr_t)x & 15) || ((uintptr_t)out & 15))
+    return fail(c, VIMA_E_INVALID, "slot_step_end: Q >= 1, E and ldx multiples of 4, 16-byte aligned fp32 rows");
+  LAUNCHED(c, launch_slot_step_end(x, ldx, S, Q, E, step_mask, len, n_valid, has_action, active, out, (cudaStream_t)stream), "slot_step_end");
 }
 
 int vima_add_pos_embed(vima_ctx* c, const float* tok, int64_t stride_b, int64_t stride_l, const int64_t* ids, const float* table, int n_pos, int B,

@@ -50,7 +50,10 @@ __global__ void __launch_bounds__(256, (D == 32) ? 2 : 1) attention_kernel(const
   constexpr int KROW = D + 8;  // padded smem row (halfs) -> conflict-free ldmatrix
   extern __shared__ __align__(16) unsigned char smem[];
   const int h = blockIdx.x, b = blockIdx.y;
-  const int Lk = p.Lk, Lq = p.Lq;
+  const int Lq = p.Lq;
+  const int qbr = p.q_batch_rows ? p.q_batch_rows : Lq;
+  int qp0, Lk;  // this batch element's (per-batch with q_pos; shared memory is sized for the capacity p.Lk)
+  attn_batch_keys(p, b, qbr, qp0, Lk);
   const int Lk_pad = (Lk + 63) & ~63;
   const int VROW = Lk_pad + 8;
   const int n_kt = Lk_pad / 64;
@@ -64,10 +67,8 @@ __global__ void __launch_bounds__(256, (D == 32) ? 2 : 1) attention_kernel(const
   float* sbias = reinterpret_cast<float*>(qb_counter + 1);     // [2*Lk-1] (log2 domain) when rel_bias
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int kvb = p.kv_batch_rows ? p.kv_batch_rows : Lk;
-  const int mld = p.mask_ld ? p.mask_ld : Lk;
-  const int qp0 = p.q_pos0;
-  const int qbr = p.q_batch_rows ? p.q_batch_rows : Lq;
+  const int kvb = p.kv_batch_rows ? p.kv_batch_rows : p.Lk;
+  const int mld = p.mask_ld ? p.mask_ld : p.Lk;
   // ---- stage K (row-major) and V (transposed) of this (b, h) in shared memory ----
   constexpr int CH = D / 8;  // 16-byte chunks per row
   for (int idx = tid; idx < Lk_pad * CH; idx += 256) {

@@ -55,12 +55,14 @@ __global__ void __launch_bounds__(TAIL_WARPS * 32) attention_tail_kernel(const A
   const long long unit = (long long)blockIdx.x * TAIL_WARPS + warp;
   if (unit >= (long long)p.B * p.H) return;  // whole warps leave; nothing below synchronises across warps
   const int b = (int)(unit / p.H), h = (int)(unit % p.H);
-  const int Lk = p.Lk;
-  const int kvb = p.kv_batch_rows ? p.kv_batch_rows : Lk;
-  const int mld = p.mask_ld ? p.mask_ld : Lk;
+  const int kvb = p.kv_batch_rows ? p.kv_batch_rows : p.Lk;
+  const int mld = p.mask_ld ? p.mask_ld : p.Lk;
   const int qbr = p.q_batch_rows ? p.q_batch_rows : p.Lq;
+  int qp0, Lk;  // this batch element's (per-batch with q_pos)
+  attn_batch_keys(p, b, qbr, qp0, Lk);
   float* qs = smt + (size_t)warp * (TAIL_NT * TAIL_D + (size_t)lk_pad * TAIL_NT);  // [8][32] queries, pre-scaled
   float* sc = qs + TAIL_NT * TAIL_D;                                                 // [lk_pad][8] scores -> weights
+  lk_pad = (Lk + 31) & ~31;  // keys this batch element walks (the shared-memory carve above keeps the launch's capacity)
 
   // ---- queries: lane = dim ----
   const float c_l2 = p.scale * LOG2E_TL;
@@ -80,7 +82,7 @@ __global__ void __launch_bounds__(TAIL_WARPS * 32) attention_tail_kernel(const A
   float mx[TAIL_NT];
 #pragma unroll
   for (int i = 0; i < TAIL_NT; ++i) mx[i] = -INFINITY;
-  const int pos0 = row0 + p.q_pos0;  // key position of tail row 0 (causal)
+  const int pos0 = row0 + qp0;  // key position of tail row 0 (causal)
   // raw (hi, lo) words of this lane's key row; the NEXT batch's rows are requested as soon as the current ones are converted, so the
   // L2 round trip overlaps the 128 packed FMAs of the batch in hand
   uint4 kh[4], kl[4];

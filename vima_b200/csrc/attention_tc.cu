@@ -76,11 +76,12 @@ __global__ void __launch_bounds__(ATC_THREADS, 2) attention_tc_kernel(const __gr
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int wg = warp >> 2;
   const int q0 = blockIdx.x * ATC_BM, h = blockIdx.y, b = blockIdx.z;
-  const int Lq = p.Lq, Lk = p.Lk;
-  const int kvb = p.kv_batch_rows ? p.kv_batch_rows : Lk;
-  const int mld = p.mask_ld ? p.mask_ld : Lk;
-  const int qp0 = p.q_pos0;
+  const int Lq = p.Lq;
+  const int kvb = p.kv_batch_rows ? p.kv_batch_rows : p.Lk;
+  const int mld = p.mask_ld ? p.mask_ld : p.Lk;
   const int qbr = p.q_batch_rows ? p.q_batch_rows : Lq;
+  int qp0, Lk;  // this batch element's (per-batch with q_pos)
+  attn_batch_keys(p, b, qbr, qp0, Lk);
   const uint32_t sbase = smem_u32(sm);
   const int rows_here = min(ATC_BM, Lq - q0);
   const int n_all = (Lk + ATC_KC - 1) / ATC_KC;

@@ -35,7 +35,19 @@ struct AttnParams {
   int mask_ld;                                 // row pitch of key_mask, 0 = Lk
   int q_pos0;                                  // causal: query row i sits at key position q_pos0 + i (incremental decode)
   int q_batch_rows;                            // rows between consecutive batch elements in q / o (>= Lq), 0 = Lq
+  const int* q_pos;                            // causal, per batch element (device, or null): position q_pos[b], keys q_pos[b] + Lq
 };
+// Causal position of query row 0 and key count of batch element b.  With q_pos the key count is q_pos[b] + (full query count of the
+// call; q_batch_rows when a body / tail split gave this launch only part of the rows), clamped to the capacity Lk.
+__device__ __forceinline__ void attn_batch_keys(const AttnParams& p, int b, int qbr, int& qp0, int& lk) {
+  if (p.q_pos == nullptr) {
+    qp0 = p.q_pos0;
+    lk = p.Lk;
+  } else {
+    qp0 = max(p.q_pos[b], 0);
+    lk = max(min(qp0 + qbr, p.Lk), 1);
+  }
+}
 constexpr int ATTN_TAIL_MAX_ROWS = 8;          // attention_tail.cu: query rows per (batch, head) the SIMT tail kernel takes
 cudaError_t launch_attention(const AttnParams& p, cudaStream_t stream);
 size_t attention_smem_bytes(const AttnParams& p);             // dynamic shared memory the mma.sync kernel needs for p
@@ -109,5 +121,14 @@ cudaError_t launch_head_select(const float* logits, int B, int n_heads, const in
 cudaError_t launch_gato_positions(const unsigned char* prompt_mask, int B, int Lp, int L, unsigned char* mask_out, long long* pos_out,
                                   cudaStream_t s);
 cudaError_t launch_max_u8(const unsigned char* x, long long n, int* out_max, cudaStream_t s);
+
+// slot decode (slots.cu)
+cudaError_t launch_slot_step_begin(const float* obs, const unsigned char* obs_mask, const float* action, int S, int Q, int E, int Lmax,
+                                   const int* len, const int* n_valid, const int* has_action, const int* active, float* tokens,
+                                   unsigned char* step_mask, long long* pos, int* q_pos, unsigned char* slot_mask, cudaStream_t s);
+cudaError_t launch_slot_kv_append(const unsigned short* qkv_hi, const unsigned short* qkv_lo, int ld_qkv, int col0, int width, int S, int Lq,
+                                  const int* q_pos, unsigned short* kv_hi, unsigned short* kv_lo, int ld_kv, int Lmax, cudaStream_t s);
+cudaError_t launch_slot_step_end(const float* x, int ldx, int S, int Q, int E, const unsigned char* step_mask, int* len, int* n_valid,
+                                 int* has_action, const int* active, float* out, cudaStream_t s);
 
 }  // namespace vima

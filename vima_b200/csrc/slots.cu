@@ -1,0 +1,122 @@
+// Slot decode (DESIGN.md 7 (f)1): every row of the batch is a slot holding one episode at its own history length, so episodes
+// are admitted and finish independently.  The per-slot state (len, n_valid, has_action, active: int32 [S]) lives on the device and
+// these three kernels read and advance it, so a step takes only by-value arguments and static shapes and captures into one CUDA
+// graph.  All three are copies, integer scans and gathers: bit-exact by construction.
+#include "kernels.h"
+
+namespace vima {
+
+// One block per slot.  Step block of L = Q+1 rows: [action, obs_1..obs_Q] once the slot has an action, else [obs_1..obs_Q, dummy]
+// (zero token, masked: causally hidden from every real row, overwritten by the next step).
+__global__ void __launch_bounds__(256) slot_step_begin_kernel(const float4* __restrict__ obs, const unsigned char* __restrict__ obs_mask,
+                                                              const float4* __restrict__ action, int Q, int E4, int Lmax,
+                                                              const int* __restrict__ len, const int* __restrict__ n_valid,
+                                                              const int* __restrict__ has_action, const int* __restrict__ active,
+                                                              float4* __restrict__ tokens, unsigned char* __restrict__ step_mask,
+                                                              long long* __restrict__ pos, int* __restrict__ q_pos,
+                                                              unsigned char* __restrict__ slot_mask) {
+  const int b = blockIdx.x, L = Q + 1;
+  const bool act = active[b] != 0, ha = has_action[b] != 0;
+  const int qp = act ? len[b] : 0;  // an inactive slot computes at column 0 of its own cache and never advances
+  const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int i = threadIdx.x; i < L * E4; i += blockDim.x) {
+    const int r = i / E4, e = i % E4;
+    float4 v = zero;
+    if (ha) v = r == 0 ? __ldg(action + (size_t)b * E4 + e) : __ldg(obs + ((size_t)b * Q + r - 1) * E4 + e);
+    else if (r < Q) v = __ldg(obs + ((size_t)b * Q + r) * E4 + e);
+    tokens[((size_t)b * L + r) * E4 + e] = v;
+  }
+  if (threadIdx.x >= 32) return;
+  const int lane = threadIdx.x;
+  const long long base = act ? (long long)n_valid[b] : 0;
+  int carry = 0;
+  for (int r0 = 0; r0 < L; r0 += 32) {
+    const int r = r0 + lane;
+    int m = 0;
+    if (r < L) m = ha ? (r == 0 ? 1 : obs_mask[(size_t)b * Q + r - 1] != 0) : (r < Q ? obs_mask[(size_t)b * Q + r] != 0 : 0);
+    int inc = m;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int y = __shfl_up_sync(0xffffffffu, inc, o);
+      if (lane >= o) inc += y;
+    }
+    if (r < L) {
+      step_mask[(size_t)b * L + r] = (unsigned char)m;
+      // position id = cumsum(mask) - 1 over the episode (a masked first token gives -1: the deferred IndexError)
+      pos[(size_t)b * L + r] = act ? base + carry + inc - 1 : 0;
+      if (qp + r < Lmax) slot_mask[(size_t)b * Lmax + qp + r] = (unsigned char)m;
+    }
+    carry += __shfl_sync(0xffffffffu, inc, 31);
+  }
+  if (lane == 0) q_pos[b] = qp;
+}
+
+cudaError_t launch_slot_step_begin(const float* obs, const unsigned char* obs_mask, const float* action, int S, int Q, int E, int Lmax,
+                                   const int* len, const int* n_valid, const int* has_action, const int* active, float* tokens,
+                                   unsigned char* step_mask, long long* pos, int* q_pos, unsigned char* slot_mask, cudaStream_t s) {
+  if (S == 0) return cudaSuccess;
+  slot_step_begin_kernel<<<S, 256, 0, s>>>(reinterpret_cast<const float4*>(obs), obs_mask, reinterpret_cast<const float4*>(action), Q, E / 4,
+                                           Lmax, len, n_valid, has_action, active, reinterpret_cast<float4*>(tokens), step_mask, pos, q_pos,
+                                           slot_mask);
+  return cudaGetLastError();
+}
+
+// Step rows (b, r) -> cache row b*Lmax + q_pos[b] + r, 8 16-bit values per thread and trip.
+__global__ void slot_kv_append_kernel(const uint4* __restrict__ qkv_hi, const uint4* __restrict__ qkv_lo, int ld_qkv8, int col8, int w8, int S,
+                                      int Lq, const int* __restrict__ q_pos, uint4* __restrict__ kv_hi, uint4* __restrict__ kv_lo, int ld_kv8,
+                                      int Lmax) {
+  const long long total = (long long)S * Lq * w8;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % w8);
+    const long long br = i / w8;
+    const int r = (int)(br % Lq), b = (int)(br / Lq);
+    const int col = q_pos[b] + r;
+    if (col < 0 || col >= Lmax) continue;
+    const size_t src = (size_t)br * ld_qkv8 + col8 + c;
+    const size_t dst = ((size_t)b * Lmax + col) * ld_kv8 + c;
+    kv_hi[dst] = __ldg(qkv_hi + src);
+    if (kv_lo) kv_lo[dst] = __ldg(qkv_lo + src);
+  }
+}
+
+cudaError_t launch_slot_kv_append(const unsigned short* qkv_hi, const unsigned short* qkv_lo, int ld_qkv, int col0, int width, int S, int Lq,
+                                  const int* q_pos, unsigned short* kv_hi, unsigned short* kv_lo, int ld_kv, int Lmax, cudaStream_t s) {
+  const long long total = (long long)S * Lq * (width / 8);
+  if (total == 0) return cudaSuccess;
+  const int blocks = (int)min((total + 255) / 256, (long long)132 * 16);
+  slot_kv_append_kernel<<<blocks, 256, 0, s>>>(reinterpret_cast<const uint4*>(qkv_hi), reinterpret_cast<const uint4*>(qkv_lo), ld_qkv / 8,
+                                               col0 / 8, width / 8, S, Lq, q_pos, reinterpret_cast<uint4*>(kv_hi),
+                                               reinterpret_cast<uint4*>(kv_lo), ld_kv / 8, Lmax);
+  return cudaGetLastError();
+}
+
+// One block per slot: gather the prediction row (Q-1 + has_action, read before the update), then advance an active slot.
+__global__ void __launch_bounds__(128) slot_step_end_kernel(const float4* __restrict__ x, int ldx4, int Q, int E4,
+                                                            const unsigned char* __restrict__ step_mask, int* __restrict__ len,
+                                                            int* __restrict__ n_valid, int* __restrict__ has_action,
+                                                            const int* __restrict__ active, float4* __restrict__ out) {
+  const int b = blockIdx.x, L = Q + 1;
+  const int ha = has_action[b] != 0;
+  const size_t row = (size_t)b * L + Q - 1 + ha;
+  for (int e = threadIdx.x; e < E4; e += blockDim.x) out[(size_t)b * E4 + e] = __ldg(x + row * ldx4 + e);
+  __syncthreads();  // every thread has read has_action[b]
+  if (threadIdx.x >= 32) return;
+  int cnt = 0;
+  for (int r = threadIdx.x; r < L; r += 32) cnt += step_mask[(size_t)b * L + r] != 0;
+  cnt = __reduce_add_sync(0xffffffffu, cnt);
+  if (threadIdx.x == 0 && active[b]) {
+    len[b] += Q + ha;
+    n_valid[b] += cnt;
+    has_action[b] = 1;
+  }
+}
+
+cudaError_t launch_slot_step_end(const float* x, int ldx, int S, int Q, int E, const unsigned char* step_mask, int* len, int* n_valid,
+                                 int* has_action, const int* active, float* out, cudaStream_t s) {
+  if (S == 0) return cudaSuccess;
+  slot_step_end_kernel<<<S, 128, 0, s>>>(reinterpret_cast<const float4*>(x), ldx / 4, Q, E / 4, step_mask, len, n_valid, has_action, active,
+                                         reinterpret_cast<float4*>(out));
+  return cudaGetLastError();
+}
+
+}  // namespace vima

@@ -18,6 +18,7 @@ from typing import Callable
 import torch
 
 from . import _C
+from . import engine as eng
 
 
 def _map(fn, x, y=None):
@@ -76,3 +77,52 @@ class GraphedStep:
     def describe(self) -> dict:
         return {"vima_kernels_per_replay": int(self.kernels_per_replay),
                 "note": "the step is captured once (torch.cuda.CUDAGraph) and replayed; inputs are copied into static buffers"}
+
+
+class GraphedSlotStep:
+    """VIMAPolicy.step_slots for one (S, Q), captured into a CUDA graph.  The slot state (len / n_valid / has_action / active) lives
+    on the device and the step's kernels read it, so admissions and releases between replays take effect.  Warm-up runs the step
+    (which advances the slots), so the state vectors and their host mirror are snapshotted first and restored afterwards; the K/V and
+    mask columns warm-up wrote lie at or past each slot's `len` and are never read before a step overwrites them.
+
+        g = policy.capture_step_slots(cache, obs, obs_mask, action)   # cache state unchanged
+        out = g(obs, obs_mask, action)                                # = policy.step_slots(cache, obs, obs_mask, action)
+    """
+
+    def __init__(self, policy, cache, obs_token: torch.Tensor, obs_mask: torch.Tensor, action_token: torch.Tensor, *, warmup: int = 2):
+        self.policy, self.cache = policy, cache
+        _, self.S, self.Q, self.E = obs_token.shape
+        cache.check_step(self.S, self.Q, self.E, eng.prec())
+        self.static_in = [obs_token.clone(), obs_mask.clone(), action_token.float().clone()]
+        dev = obs_token.device
+        self.ctx = _C.Context.get(dev)
+        saved = cache.state()
+        try:
+            side = torch.cuda.Stream(device=dev)
+            side.wait_stream(torch.cuda.current_stream(dev))
+            with torch.cuda.stream(side):
+                for _ in range(max(warmup, 1)):  # packs weights, runs the first-call host checks, sets kernel attributes
+                    policy._slot_step(cache, *self.static_in)
+            torch.cuda.current_stream(dev).wait_stream(side)
+            torch.cuda.synchronize(dev)
+            self.graph = torch.cuda.CUDAGraph()
+            n0 = self.ctx.launches
+            with torch.cuda.graph(self.graph):
+                self.static_out = policy._slot_step(cache, *self.static_in)
+            self.kernels_per_replay = self.ctx.launches - n0
+        finally:
+            cache.restore(saved)
+            torch.cuda.synchronize(dev)
+        self.replays = 0
+
+    def __call__(self, obs_token: torch.Tensor, obs_mask: torch.Tensor, action_token: torch.Tensor) -> torch.Tensor:
+        self.cache.check_step(obs_token.shape[1], obs_token.shape[2], obs_token.shape[3], eng.prec())
+        if tuple(obs_token.shape) != tuple(self.static_in[0].shape):
+            raise ValueError(f"the graph was captured for obs_token {tuple(self.static_in[0].shape)}, got {tuple(obs_token.shape)}")
+        for dst, src in zip(self.static_in, (obs_token, obs_mask, action_token)):
+            if dst.data_ptr() != src.data_ptr():
+                dst.copy_(src, non_blocking=True)
+        self.graph.replay()
+        self.replays += 1
+        self.cache.advance_host(self.Q)
+        return self.static_out

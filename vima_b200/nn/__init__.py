@@ -13,4 +13,4 @@ from .obj_encoder import (GatoMultiViewRGBEncoder, GatoViTEncoder, MultiViewRGBE
                           VisionTransformer)
 from .perceiver import ObjectsPerceiverEncoder
 from .t5_encoder import T5PromptEncoder, WordEmbedding
-from .xattn_gpt import HFGPT, DecodeCache, XAttnGPT
+from .xattn_gpt import HFGPT, DecodeCache, SlotDecodeCache, XAttnGPT

@@ -97,6 +97,68 @@ class DecodeCache:
             self.kv_lo[i].view(B, self.Lmax, 2 * E)[:, L0:L0 + Ln].copy_(qkv16.lo.view(B, Ln, -1)[:, :, E:3 * E])
 
 
+class SlotDecodeCache:
+    """K/V cache of `S` slots, each holding one episode at its own history length (DESIGN.md 4 and 7 (f)1).
+
+    Self-attention K/V per layer: `kv_hi[i]` / `kv_lo[i]` [S*Lmax, 2E]; projected prompt K/V per layer: `prompt_kv[i]` (an Opnd
+    [S*Lp_cap, 2E]) with `prompt_mask` [S, Lp_cap] (a shorter prompt's tail columns are masked).  Per-slot device state, int32 [S]:
+    `len` (cache columns used), `n_valid` (next position id), `has_action`, `active`; `q_pos` is the step's scratch copy of `len`.
+    The host mirrors len / has_action / active (it knows them from admissions and the step width), so capacity is checked without
+    reading the device."""
+
+    def __init__(self, *, S: int, Lmax: int, Lp_cap: int, E: int, n_layer: int, device, split: bool, precision: str):
+        self.S, self.Lmax, self.Lp_cap, self.E, self.precision = S, Lmax, Lp_cap, E, precision
+        mk = lambda rows: torch.zeros((rows, 2 * E), dtype=torch.int16, device=device)
+        self.kv_hi = [mk(S * Lmax) for _ in range(n_layer)]
+        self.kv_lo = [mk(S * Lmax) if split else None for _ in range(n_layer)]
+        self.prompt_kv = [eng.Opnd(S * Lp_cap, 2 * E, device, split, zero=True) for _ in range(n_layer)]
+        self.prompt_mask = torch.zeros((S, Lp_cap), dtype=torch.uint8, device=device)
+        self.mask = torch.zeros((S, Lmax), dtype=torch.uint8, device=device)
+        z = lambda: torch.zeros((S,), dtype=torch.int32, device=device)
+        self.len, self.n_valid, self.has_action, self.active, self.q_pos = z(), z(), z(), z(), z()
+        self.len_host = [0] * S
+        self.has_action_host = [False] * S
+        self.active_host = [False] * S
+
+    def slot_index(self, slots) -> list:
+        s = [int(x) for x in (slots.tolist() if isinstance(slots, torch.Tensor) else slots)]
+        if len(set(s)) != len(s) or any(not 0 <= x < self.S for x in s):
+            raise ValueError(f"slots must be distinct indices in [0, {self.S}), got {s}")
+        return s
+
+    def check_step(self, S: int, Q: int, E: int, p) -> None:
+        """Everything that can refuse a step, BEFORE any state is touched."""
+        if S != self.S or E != self.E:
+            raise ValueError(f"SlotDecodeCache(S={self.S}, E={self.E}) does not match the step's {S} slots / width {E}")
+        if Q < 1 or Q + 1 > self.Lmax:
+            raise ValueError(f"a step of {Q} obs tokens does not fit SlotDecodeCache(Lmax={self.Lmax})")
+        full = [b for b in range(self.S) if self.active_host[b] and self.len_host[b] + Q + 1 > self.Lmax]
+        if full:
+            raise ValueError(f"slots {full} cannot take {Q + 1} more tokens (Lmax={self.Lmax}, lengths {[self.len_host[b] for b in full]})")
+        self.check_precision(p)
+
+    def check_precision(self, p) -> None:
+        if self.precision != p.name:
+            raise ValueError(f"SlotDecodeCache was opened in precision mode {self.precision!r}; the current mode is {p.name!r}")
+
+    def advance_host(self, Q: int) -> None:
+        """Host mirror of what vima_slot_step_end does on the device."""
+        for b in range(self.S):
+            if self.active_host[b]:
+                self.len_host[b] += Q + int(self.has_action_host[b])
+                self.has_action_host[b] = True
+
+    def state(self) -> tuple:
+        """Copies of the per-slot state (device vectors and host mirror)."""
+        return (tuple(t.clone() for t in (self.len, self.n_valid, self.has_action, self.active)),
+                (list(self.len_host), list(self.has_action_host), list(self.active_host)))
+
+    def restore(self, st: tuple) -> None:
+        for dst, src in zip((self.len, self.n_valid, self.has_action, self.active), st[0]):
+            dst.copy_(src)
+        self.len_host, self.has_action_host, self.active_host = (list(x) for x in st[1])
+
+
 def check_cache_append(cache: "DecodeCache", B: int, L: int, E: int, p) -> None:
     """Everything that can refuse an append, BEFORE any cache state is touched (capacity, shapes, precision mode)."""
     if cache.B != B or cache.E != E:
@@ -111,7 +173,8 @@ def run_block(ctx, p, W, blk: "Block", x32, x16, c16, *, B, L, E, H, omask, chai
               layer=0):
     """GPT-1 post-LN block (components.py:23-37 / gpt.py:223-249): returns (LN2 output fp32, operands of the NEXT consumer):
     with `chain_ln` the operands are chain_ln(LN2(...)) (next layer's query LayerNorm), with `want16` they are LN2(...) itself.
-    With `cache` the L rows are the NEW tokens of each episode and attention runs over the cached prefix + themselves.
+    With `cache` (DecodeCache or SlotDecodeCache) the L rows are the NEW tokens of each episode and attention runs over the cached
+    prefix + themselves.
 
     ln_1 never runs as a kernel: c_proj's epilogue emits s = attn + x as fp32 + operands together with per-row partial sums, the
     GEGLU GEMM takes the un-normalised s with ln_1 folded into its weights (rstd / mean applied in its epilogue), and the MLP's
@@ -127,6 +190,12 @@ def run_block(ctx, p, W, blk: "Block", x32, x16, c16, *, B, L, E, H, omask, chai
         ctx.attention(q=(qkv16.hi, qkv16.lo, qkv16.ld, 0), k=(qkv16.hi, qkv16.lo, qkv16.ld, E), v=(qkv16.hi, qkv16.lo, qkv16.ld, 2 * E),
                       o=(c16.hi, c16.lo, c16.ld, 0), B=B, H=H, Lq=L, Lk=L, D=d, scale=1.0 / math.sqrt(d), causal=True, key_mask=omask,
                       dtype=p.dtype, o8=o8)
+    elif isinstance(cache, SlotDecodeCache):  # every slot at its own length: columns and causal positions from cache.q_pos
+        khi, klo = cache.kv_hi[layer], cache.kv_lo[layer]
+        ctx.slot_kv_append(qkv16.hi, qkv16.lo, qkv16.ld, E, 2 * E, B, L, cache.q_pos, khi, klo, 2 * E, cache.Lmax)
+        ctx.attention(q=(qkv16.hi, qkv16.lo, qkv16.ld, 0), k=(khi, klo, 2 * E, 0), v=(khi, klo, 2 * E, E), o=(c16.hi, c16.lo, c16.ld, 0),
+                      B=B, H=H, Lq=L, Lk=cache.Lmax, D=d, scale=1.0 / math.sqrt(d), causal=True, key_mask=cache.mask, dtype=p.dtype, o8=o8,
+                      kv_batch_rows=cache.Lmax, mask_ld=cache.Lmax, q_pos=cache.q_pos)
     else:
         L0 = cache.L
         cache.append_kv(layer, qkv16, L0, L)
@@ -308,6 +377,53 @@ class XAttnGPT(nn.Module):
             assert torch.all(obs_action_masks.sum(dim=-1) > 0)
             assert obs_action_masks.dtype == torch.bool
 
+    def _prompt_operand(self, ctx, p, prompt_tokens, prompt_position_ids, batch_first, B, Lp, E, err) -> "eng.Opnd":
+        """prompt + xattn_positions_embed[ids], the key_value GEMM's operand [B*Lp, E] (out-of-range ids set `err`)."""
+        dev = prompt_tokens.device
+        ptk = prompt_tokens if prompt_tokens.stride(-1) == 1 else prompt_tokens.contiguous()
+        psb, psl = (ptk.stride(0), ptk.stride(1)) if batch_first else (ptk.stride(1), ptk.stride(0))
+        if prompt_position_ids is None:
+            prompt_position_ids = self.xattn_position_ids[None, :Lp].expand(B, Lp)
+        pr_ids = prompt_position_ids.to(torch.int64).contiguous()
+        Mp = B * Lp
+        kv16 = eng.Opnd(Mp, E, dev, p.split, f8=p.f8)
+        if p.f8:  # prompt + position embedding feeds only the key_value GEMM: fp32 once, then hi16 + e4m3 views
+            kv32 = torch.empty((Mp, E), dtype=torch.float32, device=dev)
+            ctx.add_pos_embed(ptk, psb, psl, pr_ids, self.xattn_positions_embed.weight.detach(), B, Lp, E, out_f32=kv32, hi=kv16.hi, lo=None,
+                              dtype=p.dtype, err_flag=err)
+            ctx.split_f8(kv32, kv16.lo8, kv16.hi8)
+            del kv32
+        else:
+            ctx.add_pos_embed(ptk, psb, psl, pr_ids, self.xattn_positions_embed.weight.detach(), B, Lp, E, hi=kv16.hi, lo=kv16.lo,
+                              dtype=p.dtype, err_flag=err)
+        return kv16
+
+    @torch.no_grad()
+    def admit_prompts(self, cache: SlotDecodeCache, slots: list, prompt_tokens: torch.Tensor, prompt_mask_u8: torch.Tensor,
+                      prompt_position_ids: torch.Tensor) -> None:
+        """Projected prompt keys/values of every layer for the n new prompts only (prompt_tokens (Lp,n,E), mask / position ids (n,Lp)),
+        scattered into `slots` of the cache; their prompt masks are padded to Lp_cap with masked columns and their state is reset to
+        an empty history.  The caller has validated shapes, slots and the precision mode."""
+        ctx = eng.ctx_for(prompt_tokens)
+        p = eng.prec()
+        Lp, n, E = prompt_tokens.shape
+        dev = prompt_tokens.device
+        self._pos_guard.poll()
+        err = self._pos_guard.device_flag(dev)  # a bad prompt position id is reported by the next step
+        kv16 = self._prompt_operand(ctx, p, prompt_tokens.float(), prompt_position_ids, False, n, Lp, E, err)
+        idx = torch.tensor(slots, dtype=torch.int64, device=dev)
+        for W, dst in zip(self._packed(ctx, p), cache.prompt_kv):
+            kv = eng.gemm(ctx, kv16, W["wkv"], p, want16=True)[1]
+            for d_t, s_t in ((dst.hi, kv.hi), (dst.lo, kv.lo)):
+                if d_t is not None:
+                    d_t.view(cache.S, cache.Lp_cap, -1)[idx, :Lp] = s_t[: n * Lp].view(n, Lp, -1)
+        cache.prompt_mask[idx] = 0
+        cache.prompt_mask[idx, :Lp] = prompt_mask_u8
+        for t, v in ((cache.len, 0), (cache.n_valid, 0), (cache.has_action, 0), (cache.active, 1)):
+            t[idx] = v
+        for b in slots:
+            cache.len_host[b], cache.has_action_host[b], cache.active_host[b] = 0, False, True
+
     # ---------------------------------------------------------------------------------------------
     def forward(
         self,
@@ -319,47 +435,53 @@ class XAttnGPT(nn.Module):
         prompt_position_ids: Optional[torch.Tensor] = None,
         batch_first: bool = False,
         obs_action_masks: Optional[torch.Tensor] = None,
-        cache: Optional[DecodeCache] = None,
+        cache=None,
     ):
         """Reference signature (xattn_gpt.py:89-99) plus `cache`: with a DecodeCache the obs/action arguments describe only the
-        tokens appended this step (their position ids are absolute) and the return value holds only their rows."""
+        tokens appended this step (their position ids are absolute) and the return value holds only their rows.  With a
+        SlotDecodeCache they are one step block per slot as vima_slot_step_begin lays it out (the slots' prompts are in the cache;
+        `prompt_tokens` is not read)."""
         ctx = eng.ctx_for(obs_action_tokens)
         p = eng.prec()
+        slots = isinstance(cache, SlotDecodeCache)
         if not self._input_checked and cache is None:
             self._check_input(obs_action_tokens, prompt_tokens, prompt_mask, batch_first, obs_action_masks)
         dev = obs_action_tokens.device
         if batch_first:
             B, L, E = obs_action_tokens.shape
-            Lp = prompt_tokens.shape[1]
         else:
             L, B, E = obs_action_tokens.shape
-            Lp = prompt_tokens.shape[0]
+        if slots:
+            Lp = cache.Lp_cap
+        else:
+            Lp = prompt_tokens.shape[1] if batch_first else prompt_tokens.shape[0]
         assert E == self.embd_dim
         assert Lp <= self.xattn_n_positions and L <= self.n_positions
         if cache is not None:
             if obs_action_position_ids is None or obs_action_masks is None:
                 raise ValueError("cached decode needs absolute position ids and masks for the appended tokens")
-            check_cache_append(cache, B, L, E, p)
-        if obs_action_tokens.dtype != torch.float32 or prompt_tokens.dtype != torch.float32:
+            if slots:
+                cache.check_step(B, L - 1, E, p)
+            else:
+                check_cache_append(cache, B, L, E, p)
+        if obs_action_tokens.dtype != torch.float32 or (not slots and prompt_tokens.dtype != torch.float32):
             raise TypeError("XAttnGPT expects float32 tokens (xattn_gpt.py:150,152)")
         tok = obs_action_tokens if obs_action_tokens.stride(-1) == 1 else obs_action_tokens.contiguous()
-        ptk = prompt_tokens if prompt_tokens.stride(-1) == 1 else prompt_tokens.contiguous()
         sb, sl = (tok.stride(0), tok.stride(1)) if batch_first else (tok.stride(1), tok.stride(0))
-        psb, psl = (ptk.stride(0), ptk.stride(1)) if batch_first else (ptk.stride(1), ptk.stride(0))
         if obs_action_position_ids is None:
             obs_action_position_ids = self.position_ids[None, :L].expand(B, L)
-        if prompt_position_ids is None:
-            prompt_position_ids = self.xattn_position_ids[None, :Lp].expand(B, Lp)
         oa_ids = obs_action_position_ids.to(torch.int64).contiguous()
-        pr_ids = prompt_position_ids.to(torch.int64).contiguous()
         if prompt_mask is not None and prompt_mask.dim() == 3:
             prompt_mask = prompt_mask.squeeze(1)
-        pmask = None if prompt_mask is None else eng.as_u8(prompt_mask)
+        if slots:
+            pmask = cache.prompt_mask
+        else:
+            pmask = None if prompt_mask is None else eng.as_u8(prompt_mask)
         omask = None if obs_action_masks is None else eng.as_u8(obs_action_masks)
-        if cache is not None:
+        if cache is not None and not slots:  # (the slot step's mask columns are written by vima_slot_step_begin)
             cache.mask[:, cache.L:cache.L + L].copy_(omask)
 
-        M, Mp, H, Hx = B * L, B * Lp, self.n_head, self.xattn_n_head
+        M, H, Hx = B * L, self.n_head, self.xattn_n_head
         d_s, d_x = E // H, E // Hx
         self._pos_guard.poll()
         err = self._pos_guard.device_flag(dev)
@@ -367,18 +489,7 @@ class XAttnGPT(nn.Module):
         x32 = torch.empty((M, E), dtype=torch.float32, device=dev)
         ctx.add_pos_embed(tok, sb, sl, oa_ids, self.positions_embed.weight.detach(), B, L, E, out_f32=x32, err_flag=err)
         need_prompt = cache is None or cache.prompt_kv is None
-        kv16 = eng.Opnd(Mp, E, dev, p.split, f8=p.f8) if need_prompt else None
-        if not need_prompt:
-            pass
-        elif p.f8:  # prompt + position embedding feeds only the key_value GEMM: fp32 once, then hi16 + e4m3 views
-            kv32 = torch.empty((Mp, E), dtype=torch.float32, device=dev)
-            ctx.add_pos_embed(ptk, psb, psl, pr_ids, self.xattn_positions_embed.weight.detach(), B, Lp, E, out_f32=kv32, hi=kv16.hi, lo=None,
-                              dtype=p.dtype, err_flag=err)
-            ctx.split_f8(kv32, kv16.lo8, kv16.hi8)
-            del kv32
-        else:
-            ctx.add_pos_embed(ptk, psb, psl, pr_ids, self.xattn_positions_embed.weight.detach(), B, Lp, E, hi=kv16.hi, lo=kv16.lo,
-                              dtype=p.dtype, err_flag=err)
+        kv16 = self._prompt_operand(ctx, p, prompt_tokens, prompt_position_ids, batch_first, B, Lp, E, err) if need_prompt else None
         self._pos_guard.after_launch()  # first call: synchronous check; later: asynchronous copy, reported by the next call
         if cache is None:
             self._input_checked = True
@@ -408,7 +519,7 @@ class XAttnGPT(nn.Module):
             nxt = self.xattns[i + 1].layernorm if i + 1 < self.n_layer else None
             x32, qin16 = run_block(ctx, p, W, blk, xb32, xb16, c16, B=B, L=L, E=E, H=H, omask=omask, chain_ln=nxt, out_f32=x32, cache=cache,
                                    layer=i)
-        if cache is not None:
+        if cache is not None and not slots:
             cache.L += L
         out = x32.view(B, L, E)
         return out if batch_first else out.transpose(0, 1)

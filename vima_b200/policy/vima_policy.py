@@ -135,6 +135,90 @@ class VIMAPolicy(nn.Module):
         return out[-1:]
 
     # --------------------------------------------------------------------------------------------------
+    # Slot decode (DESIGN.md 7 (f)1): each row of the batch is a slot holding one episode at a time, so episodes start and finish
+    # independently (a vectorised environment resets each of its environments on its own).
+    def open_slots(self, n_slots: int, *, max_tokens: Optional[int] = None, max_prompt_tokens: int = 256):
+        """Allocate a SlotDecodeCache of `n_slots` slots (all inactive) with room for `max_tokens` history tokens (default: the
+        decoder's n_positions) and `max_prompt_tokens` prompt tokens per episode, in the current precision mode."""
+        dev = self.xattn_gpt.positions_embed.weight.device
+        eng.ctx_for(self.xattn_gpt.positions_embed.weight)
+        Lmax = self.xattn_gpt.n_positions if max_tokens is None else int(max_tokens)
+        if not 1 < Lmax <= self.xattn_gpt.n_positions:
+            raise ValueError(f"max_tokens={Lmax} outside (1, n_positions={self.xattn_gpt.n_positions}]")
+        if not 0 < max_prompt_tokens <= self.xattn_gpt.xattn_n_positions:
+            raise ValueError(f"max_prompt_tokens={max_prompt_tokens} outside (0, {self.xattn_gpt.xattn_n_positions}]")
+        if n_slots < 1:
+            raise ValueError("n_slots must be >= 1")
+        p = eng.prec()
+        return vnn.SlotDecodeCache(S=int(n_slots), Lmax=Lmax, Lp_cap=int(max_prompt_tokens), E=self.embed_dim, n_layer=self.xattn_gpt.n_layer,
+                                   device=dev, split=p.split, precision=p.name)
+
+    def admit(self, cache, slots, prompt_token: torch.Tensor, prompt_token_mask: torch.Tensor) -> None:
+        """Start a new episode in each of `slots` (replacing whatever they held): prompt_token (Lp,n,E), prompt_token_mask (n,Lp),
+        Lp <= the cache's max_prompt_tokens.  Runs the prompt key/value GEMMs of the n prompts only, on the current stream."""
+        s = cache.slot_index(slots)
+        Lp, n, E = prompt_token.shape
+        if n != len(s) or E != cache.E or tuple(prompt_token_mask.shape) != (n, Lp):
+            raise ValueError(f"admit: {len(s)} slots need prompt_token (Lp, {len(s)}, {cache.E}) and a ({len(s)}, Lp) mask, got "
+                             f"{tuple(prompt_token.shape)} / {tuple(prompt_token_mask.shape)}")
+        if Lp > cache.Lp_cap:
+            raise ValueError(f"admit: prompt of {Lp} tokens exceeds the cache's max_prompt_tokens={cache.Lp_cap}")
+        cache.check_precision(eng.prec())
+        if not s:
+            return
+        ctx = eng.ctx_for(prompt_token)
+        pmask_u8 = eng.as_u8(prompt_token_mask)
+        prompt_pos = torch.empty(pmask_u8.shape, dtype=torch.int64, device=prompt_token.device)
+        ctx.mask_cumsum(pmask_u8, prompt_pos)
+        self.xattn_gpt.admit_prompts(cache, s, prompt_token, pmask_u8, prompt_pos)
+
+    def release(self, cache, slots) -> None:
+        """Mark `slots` inactive (their episodes ended); they keep computing on whatever is passed but never advance."""
+        s = cache.slot_index(slots)
+        if s:
+            cache.active[torch.tensor(s, dtype=torch.int64, device=cache.active.device)] = 0
+        for b in s:
+            cache.active_host[b] = False
+
+    def step_slots(self, cache, obs_token: torch.Tensor, obs_mask: torch.Tensor, action_token: Optional[torch.Tensor]) -> torch.Tensor:
+        """One environment step of every slot: obs_token (1,S,Q,E), obs_mask (1,S,Q), action_token (1,S,E) (the previous action of
+        each slot; ignored for slots at their first step; None = all zeros) -> predicted action token (1,S,E).  For an active slot
+        the row equals `forward(...)[-1:]` at B=1 over that episode's own history; an inactive slot's row is unspecified."""
+        _, S, Q, E = obs_token.shape
+        cache.check_step(S, Q, E, eng.prec())  # every refusal happens before any state is touched
+        out = self._slot_step(cache, obs_token, obs_mask, action_token)
+        cache.advance_host(Q)
+        return out
+
+    def _slot_step(self, cache, obs_token, obs_mask, action_token):
+        """The device side of `step_slots`: static shapes for a fixed (S, Q), no host synchronisation (captured by GraphedSlotStep)."""
+        ctx = eng.ctx_for(obs_token)
+        _, S, Q, E = obs_token.shape
+        dev = obs_token.device
+        L = Q + 1
+        obs = obs_token[0].float().contiguous()
+        m = eng.as_u8(obs_mask[0])
+        act = torch.zeros((S, E), dtype=torch.float32, device=dev) if action_token is None else action_token[0].float().contiguous()
+        tokens = torch.empty((S * L, E), dtype=torch.float32, device=dev)
+        step_mask = torch.empty((S, L), dtype=torch.uint8, device=dev)
+        pos = torch.empty((S, L), dtype=torch.int64, device=dev)
+        ctx.slot_step_begin(obs, m, act, Lmax=cache.Lmax, len_=cache.len, n_valid=cache.n_valid, has_action=cache.has_action,
+                            active=cache.active, tokens=tokens, step_mask=step_mask, pos=pos, q_pos=cache.q_pos, slot_mask=cache.mask)
+        x = self.xattn_gpt(obs_action_tokens=tokens.view(S, L, E), obs_action_position_ids=pos, prompt_tokens=None,
+                           obs_action_masks=step_mask.view(torch.bool), batch_first=True, cache=cache)
+        out = torch.empty((S, E), dtype=torch.float32, device=dev)
+        ctx.slot_step_end(x.reshape(S * L, E), S, Q, E, step_mask, len_=cache.len, n_valid=cache.n_valid, has_action=cache.has_action,
+                          active=cache.active, out=out)
+        return out.view(1, S, E)
+
+    def capture_step_slots(self, cache, obs_token: torch.Tensor, obs_mask: torch.Tensor, action_token: torch.Tensor, *, warmup: int = 2):
+        """`step_slots` for this (S, Q) captured into one CUDA graph (vima_b200.graphs.GraphedSlotStep); the cache's slot state is
+        left as it was.  Call the result like step_slots without the cache: g(obs_token, obs_mask, action_token)."""
+        from ..graphs import GraphedSlotStep
+
+        return GraphedSlotStep(self, cache, obs_token, obs_mask, action_token, warmup=warmup)
+
+    # --------------------------------------------------------------------------------------------------
     def forward_prompt_assembly(self, prompts):
         """(token_types, word_batch, image_batch) -> prompt tokens (Lp,B,E), masks (B,Lp) bool  (vima_policy.py:161-240)."""
         raw_prompts_token_type, word_batch, image_batch = prompts
