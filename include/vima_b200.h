@@ -252,6 +252,15 @@ int vima_slot_kv_append(vima_ctx*, const void* qkv_hi, const void* qkv_lo, int l
  * n_valid += sum(step_mask[b]), has_action = 1. */
 int vima_slot_step_end(vima_ctx*, const float* x, int ldx, int S, int Q, int E, const uint8_t* step_mask, int32_t* len, int32_t* n_valid,
                        int32_t* has_action, const int32_t* active, float* out, void* stream);
+/* Decoder-only admission (VIMA-Gato / VIMA-GPT: prompt + separator live in the self-attention cache).  Per layer: columns
+ * [col0, col0 + width) of the prefill rows qkv [n*Lq, ld_qkv] (hi, lo|NULL 16-bit) -> cache rows slots[j]*Lmax + r (r < Lq) of
+ * kv [S*Lmax, ld_kv]; slots: DEVICE int32 [n], distinct.  Lq <= Lmax; width, col0, ld_* multiples of 8 elements, 16-byte aligned. */
+int vima_slot_kv_scatter(vima_ctx*, const void* qkv_hi, const void* qkv_lo, int ld_qkv, int col0, int width, int n, int Lq, const int32_t* slots,
+                         void* kv_hi, void* kv_lo, int ld_kv, int Lmax, void* stream);
+/* For each admitted slot b = slots[j] (DEVICE int32 [n]): slot_mask[b, 0:Lp] = prompt_mask[j] (uint8 [n, Lp]), slot_mask[b, Lp] = 1;
+ * len[b] = Lp+1, n_valid[b] = sum(prompt_mask[j] != 0) + 1, has_action[b] = 0, active[b] = 1.  Lp + 1 <= Lmax. */
+int vima_slot_admit_prefix(vima_ctx*, const int32_t* slots, int n, const uint8_t* prompt_mask, int Lp, int Lmax, uint8_t* slot_mask,
+                           int32_t* len, int32_t* n_valid, int32_t* has_action, int32_t* active, void* stream);
 /* out[b,l,:] = tok[b*stride_b + l*stride_l + :] + table[ids[b,l]]  (xattn_gpt.py:103-105,110-114); out-of-range
  * ids set *err_flag (device int) to 1 -- the reference raises IndexError there. */
 int vima_add_pos_embed(vima_ctx*, const float* tok, int64_t stride_b, int64_t stride_l, const int64_t* ids, const float* table, int n_pos,

@@ -1,5 +1,11 @@
 """Slot decode vs lockstep decode in a simulated vectorised environment (cfg3 shapes: 200M, 256 slots, Q = 32 obs tokens, Lp = 256).
 
+With --policy gato | gpt | flamingo the same simulation runs on a baseline policy (e.g. `--policy gato --model gato_200M`: cfg5
+shapes, 22 layers, Q = 16 tokens per observation).  The decoder-only baselines hold prompt + separator in the cache, so a slot has
+Lp + 1 + --max-steps * (Q + 1) columns (512 at cfg5), and a fourth run is added in front:
+
+  reforward  forward over the whole growing history every step, as the reference's env loop does (episodes in batches of --slots)
+
 Episode lengths are drawn from a seeded uniform distribution over 1..--max-steps environment steps (15 * 33 tokens fit the 512
 positions).  Every episode runs to its end in each of three runs, and each run reports completed env-steps/s and episodes/s:
 
@@ -36,7 +42,8 @@ def gpu_info() -> str:
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--model", default="200M")
+    ap.add_argument("--policy", default="vima", choices=["vima", "gato", "gpt", "flamingo"])
+    ap.add_argument("--model", default=None, help="synth config name (default: 200M for vima, gato_200M for gato / gpt, flamingo_tiny)")
     ap.add_argument("--slots", type=int, default=256)
     ap.add_argument("--n-obj", type=int, default=32)
     ap.add_argument("--prompt-len", type=int, default=256)
@@ -44,27 +51,69 @@ def main():
     ap.add_argument("--episodes", type=int, default=1024)
     ap.add_argument("--precision", default="f16f8")
     ap.add_argument("--seed", type=int, default=0)
-    ap.add_argument("--runs", default="lockstep,eager,graph")
+    ap.add_argument("--runs", default=None, help="default: lockstep,eager,graph (vima); reforward,lockstep,eager,graph (baselines)")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("slot_decode_bench needs a CUDA device")
     vima_b200.set_precision(a.precision)
     torch.manual_seed(a.seed)
-    pol = vima_b200.VIMAPolicy(**synth.MODEL_CFGS[a.model]).cuda().eval()
-    E, S, Q, Lp = pol.embed_dim, a.slots, a.n_obj, a.prompt_len
-    Lmax = a.max_steps * (Q + 1)
+    vima = a.policy == "vima"
+    if vima:
+        pol = vima_b200.VIMAPolicy(**synth.MODEL_CFGS[a.model or "200M"]).cuda().eval()
+    elif a.policy == "flamingo":
+        pol = vima_b200.VIMAFlamingoPolicy(**synth.FLAMINGO_CFGS[a.model or "flamingo_tiny"]).cuda().eval()
+    else:
+        cls = vima_b200.VIMAGatoPolicy if a.policy == "gato" else vima_b200.VIMAGPTPolicy
+        pol = cls(**synth.GATO_CFGS[a.model or "gato_200M"]).cuda().eval()
+    E, S, Lp = pol.embed_dim, a.slots, a.prompt_len
+    Q = a.n_obj if vima else pol._obj_xf_num_queries
+    prefix = Lp + 1 if a.policy in ("gato", "gpt") else 0  # the decoder-only caches hold prompt + separator
+    Lmax = prefix + a.max_steps * (Q + 1)
+    runs = (a.runs or ("lockstep,eager,graph" if vima else "reforward,lockstep,eager,graph")).split(",")
     lengths = np.random.default_rng(a.seed).integers(1, a.max_steps + 1, size=a.episodes).tolist()
     total_steps = int(sum(lengths))
     g = torch.Generator(device="cuda").manual_seed(a.seed)
-    obs_pool = [torch.randn(1, S, Q, E, device="cuda", generator=g) for _ in range(3)]
+    obs_shape = (1, S, E) if a.policy == "gpt" else (1, S, Q, E)
+    obs_pool = [torch.randn(*obs_shape, device="cuda", generator=g) for _ in range(3)]
     msk = torch.rand(1, S, Q, device="cuda", generator=g) > 0.1
     msk[..., 0] = True
     act = torch.randn(1, S, E, device="cuda", generator=g)
     prompts = torch.randn(Lp, S, E, device="cuda", generator=g)
     pmask = torch.ones(S, Lp, dtype=torch.bool, device="cuda")
     info = gpu_info()
-    print(f"# {info}; model {a.model}, {S} slots, Q={Q}, Lp={Lp}, {a.precision}; {a.episodes} episodes of 1..{a.max_steps} steps "
+    name = "" if vima else f"policy {a.policy}, "
+    print(f"# {info}; {name}model {a.model or '200M'}, {S} slots, Q={Q}, Lp={Lp}, {a.precision}; {a.episodes} episodes of 1..{a.max_steps} steps "
           f"({total_steps} env-steps, seed {a.seed})")
+
+    if vima:
+        forward_step, step_slots = pol.forward_step, pol.step_slots
+        open_slots = lambda: pol.open_slots(S, max_tokens=Lmax, max_prompt_tokens=Lp)  # noqa: E731
+        capture = pol.capture_step_slots
+        replay = lambda gs, o, m, x: gs(o, m, x)  # noqa: E731
+    else:
+        forward_step = lambda c, o, m, x: pol.forward_step(c, o, x)  # noqa: E731
+        step_slots = lambda c, o, m, x: pol.step_slots(c, o, x)  # noqa: E731
+        open_slots = lambda: pol.open_slots(S, max_tokens=Lmax)  # noqa: E731
+        capture = lambda c, o, m, x: pol.capture_step_slots(c, o, x)  # noqa: E731
+        replay = lambda gs, o, m, x: gs(o, x)  # noqa: E731
+
+    def reforward():
+        """forward over the whole history at every step (episodes in batches of S, a batch runs until its longest episode ends)."""
+        obs_hist = torch.cat([obs_pool[t % 3] for t in range(a.max_steps)], 0)
+        msk_hist = msk.expand(a.max_steps, *msk.shape[1:])
+        act_hist = act.expand(a.max_steps, *act.shape[1:])
+        ticks = 0
+        for i in range(0, len(lengths), S):
+            batch = lengths[i:i + S]
+            n = len(batch)
+            for t in range(max(batch)):
+                at = None if t == 0 else act_hist[:t, :n]
+                if vima:
+                    pol.forward(obs_hist[:t + 1, :n], msk_hist[:t + 1, :n], at, prompts[:, :n], pmask[:n])
+                else:
+                    pol.forward(obs_hist[:t + 1, :n], at, prompts[:, :n], pmask[:n])
+                ticks += 1
+        return ticks, 0.0
 
     def lockstep():
         ticks = 0
@@ -73,7 +122,7 @@ def main():
             n = len(batch)
             cache = pol.start_decode(prompts[:, :n], pmask[:n], max_tokens=Lmax)
             for t in range(max(batch)):
-                pol.forward_step(cache, obs_pool[t % 3][:, :n], msk[:, :n], None if t == 0 else act[:, :n])
+                forward_step(cache, obs_pool[t % 3][:, :n], msk[:, :n], None if t == 0 else act[:, :n])
                 ticks += 1
         return ticks, 0.0
 
@@ -109,35 +158,36 @@ def main():
         torch.cuda.synchronize()
         return ticks, sum(e0.elapsed_time(e1) for e0, e1 in adm_ms)
 
-    runs = a.runs.split(",")
     results = []
     with torch.no_grad():
         # warm-up: modules, weight packing, kernel attributes
-        c = pol.open_slots(S, max_tokens=Lmax, max_prompt_tokens=Lp)
+        c = open_slots()
         pol.admit(c, list(range(S)), prompts, pmask)
         for _ in range(2):
-            pol.step_slots(c, obs_pool[0], msk, act)
+            step_slots(c, obs_pool[0], msk, act)
         cd = pol.start_decode(prompts, pmask, max_tokens=Lmax)
         for t in range(2):
-            pol.forward_step(cd, obs_pool[0], msk, None if t == 0 else act)
+            forward_step(cd, obs_pool[0], msk, None if t == 0 else act)
         del c, cd
         torch.cuda.synchronize()
         for name in runs:
             extra = {}
-            if name == "lockstep":
+            if name == "reforward":
+                fn = reforward
+            elif name == "lockstep":
                 fn = lockstep
             elif name == "eager":
-                cache = pol.open_slots(S, max_tokens=Lmax, max_prompt_tokens=Lp)
-                fn = lambda: slotted(pol.step_slots, cache)  # noqa: E731
+                cache = open_slots()
+                fn = lambda: slotted(step_slots, cache)  # noqa: E731
             elif name == "graph":
-                cache = pol.open_slots(S, max_tokens=Lmax, max_prompt_tokens=Lp)
+                cache = open_slots()
                 pol.admit(cache, list(range(S)), prompts, pmask)
                 t0 = time.perf_counter()
-                gs = pol.capture_step_slots(cache, obs_pool[0], msk, act)
+                gs = capture(cache, obs_pool[0], msk, act)
                 torch.cuda.synchronize()
                 extra = {"capture_s": round(time.perf_counter() - t0, 3), "vima_kernels_per_replay": gs.kernels_per_replay}
                 pol.release(cache, list(range(S)))
-                fn = lambda: slotted(lambda c, o, m, x: gs(o, m, x), cache)  # noqa: E731
+                fn = lambda: slotted(lambda c, o, m, x: replay(gs, o, m, x), cache)  # noqa: E731
             else:
                 raise SystemExit(f"unknown run {name}")
             torch.cuda.synchronize()
@@ -147,7 +197,7 @@ def main():
             dt = time.perf_counter() - t0
             r = {"run": name, "seconds": round(dt, 4), "ticks": ticks, "env_steps_per_s": round(total_steps / dt, 1),
                  "episodes_per_s": round(len(lengths) / dt, 2), "ms_per_tick": round(dt * 1e3 / ticks, 3)}
-            if name != "lockstep":
+            if name not in ("lockstep", "reforward"):
                 r["admission_ms_total"] = round(adm, 2)
                 r["admission_ms_per_episode"] = round(adm / len(lengths), 4)
             r.update(extra)

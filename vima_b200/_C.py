@@ -95,7 +95,7 @@ EXPORTS = [
     "vima_attention", "vima_small_attention", "vima_assemble_history", "vima_mask_cumsum", "vima_add_pos_embed",
     "vima_gather_prompt", "vima_patchify", "vima_vit_tokens", "vima_bbox_norm", "vima_fill_ee", "vima_max_u8",
     "vima_action_scale", "vima_action_postprocess", "vima_latent_attention", "vima_object_stats", "vima_crop_resize", "vima_head_select", "vima_gato_positions", "vima_pack_weight_f8", "vima_split_f8",
-    "vima_slot_step_begin", "vima_slot_kv_append", "vima_slot_step_end",
+    "vima_slot_step_begin", "vima_slot_kv_append", "vima_slot_step_end", "vima_slot_kv_scatter", "vima_slot_admit_prefix",
 ]
 
 
@@ -334,6 +334,22 @@ class Context:
         self._ck(self.lib.vima_slot_step_end(self.h, c_void_p(x.data_ptr()), x.stride(0), int(S), int(Q), int(E), c_void_p(step_mask.data_ptr()),
                                              c_void_p(len_.data_ptr()), c_void_p(n_valid.data_ptr()), c_void_p(has_action.data_ptr()),
                                              c_void_p(active.data_ptr()), c_void_p(out.data_ptr()), c_void_p(self._s())), "slot_step_end")
+
+    def slot_kv_scatter(self, qkv_hi, qkv_lo, ld_qkv, col0, width, n, Lq, slots, kv_hi, kv_lo, ld_kv, Lmax):
+        """Prefill rows (j, r) of qkv [n*Lq, ld_qkv], columns [col0, col0+width) -> rows slots[j]*Lmax + r of kv; slots int32 [n]."""
+        assert slots.dtype == torch.int32 and slots.is_contiguous() and slots.numel() >= n
+        self._ck(self.lib.vima_slot_kv_scatter(self.h, c_void_p(qkv_hi.data_ptr()), c_void_p(_ptr(qkv_lo)), int(ld_qkv), int(col0), int(width),
+                                               int(n), int(Lq), c_void_p(slots.data_ptr()), c_void_p(kv_hi.data_ptr()), c_void_p(_ptr(kv_lo)),
+                                               int(ld_kv), int(Lmax), c_void_p(self._s())), "slot_kv_scatter")
+
+    def slot_admit_prefix(self, slots, prompt_mask_u8, Lmax, slot_mask, *, len_, n_valid, has_action, active):
+        """slots int32 [n], prompt_mask uint8 [n, Lp] -> mask columns [0, Lp] of the admitted slots and their fresh state."""
+        n, Lp = prompt_mask_u8.shape
+        assert slots.dtype == torch.int32 and slots.numel() == n and prompt_mask_u8.is_contiguous()
+        self._ck(self.lib.vima_slot_admit_prefix(self.h, c_void_p(slots.data_ptr()), int(n), c_void_p(prompt_mask_u8.data_ptr()), int(Lp), int(Lmax),
+                                                 c_void_p(slot_mask.data_ptr()), c_void_p(len_.data_ptr()), c_void_p(n_valid.data_ptr()),
+                                                 c_void_p(has_action.data_ptr()), c_void_p(active.data_ptr()), c_void_p(self._s())),
+                 "slot_admit_prefix")
 
     def add_pos_embed(self, tok, stride_b, stride_l, ids, table, B, L, E, *, out_f32=None, hi=None, lo=None, dtype=DT_F16, err_flag=None):
         self._ck(self.lib.vima_add_pos_embed(self.h, c_void_p(tok.data_ptr()), c_i64(stride_b), c_i64(stride_l), c_void_p(ids.data_ptr()),

@@ -496,6 +496,29 @@ int vima_slot_step_end(vima_ctx* c, const float* x, int ldx, int S, int Q, int E
   LAUNCHED(c, launch_slot_step_end(x, ldx, S, Q, E, step_mask, len, n_valid, has_action, active, out, (cudaStream_t)stream), "slot_step_end");
 }
 
+int vima_slot_kv_scatter(vima_ctx* c, const void* qkv_hi, const void* qkv_lo, int ld_qkv, int col0, int width, int n, int Lq, const int32_t* slots,
+                         void* kv_hi, void* kv_lo, int ld_kv, int Lmax, void* stream) {
+  CHECK_CTX(c);
+  if (!qkv_hi || !kv_hi || !slots || (qkv_lo == nullptr) != (kv_lo == nullptr)) return fail(c, VIMA_E_INVALID, "slot_kv_scatter: null pointer");
+  auto al = [](const void* q) { return ((uintptr_t)q & 15) == 0; };
+  if ((ld_qkv & 7) || (col0 & 7) || (width & 7) || (ld_kv & 7) || width <= 0 || col0 < 0 || col0 + width > ld_qkv || width > ld_kv || n < 0 ||
+      Lq < 1 || Lq > Lmax || !al(qkv_hi) || !al(qkv_lo) || !al(kv_hi) || !al(kv_lo))
+    return fail(c, VIMA_E_INVALID, "slot_kv_scatter: ld / col0 / width multiples of 8 inside the rows, 16-byte aligned bases, 1 <= Lq <= Lmax");
+  LAUNCHED(c, launch_slot_kv_scatter((const unsigned short*)qkv_hi, (const unsigned short*)qkv_lo, ld_qkv, col0, width, n, Lq, slots,
+                                     (unsigned short*)kv_hi, (unsigned short*)kv_lo, ld_kv, Lmax, (cudaStream_t)stream),
+           "slot_kv_scatter");
+}
+
+int vima_slot_admit_prefix(vima_ctx* c, const int32_t* slots, int n, const uint8_t* prompt_mask, int Lp, int Lmax, uint8_t* slot_mask,
+                           int32_t* len, int32_t* n_valid, int32_t* has_action, int32_t* active, void* stream) {
+  CHECK_CTX(c);
+  if (!slots || !prompt_mask || !slot_mask || !len || !n_valid || !has_action || !active)
+    return fail(c, VIMA_E_INVALID, "slot_admit_prefix: null pointer");
+  if (n < 0 || Lp < 0 || Lp + 1 > Lmax) return fail(c, VIMA_E_INVALID, "slot_admit_prefix: n >= 0, 0 <= Lp, Lp + 1 <= Lmax");
+  LAUNCHED(c, launch_slot_admit_prefix(slots, n, prompt_mask, Lp, Lmax, slot_mask, len, n_valid, has_action, active, (cudaStream_t)stream),
+           "slot_admit_prefix");
+}
+
 int vima_add_pos_embed(vima_ctx* c, const float* tok, int64_t stride_b, int64_t stride_l, const int64_t* ids, const float* table, int n_pos, int B,
                        int L, int E, float* out_f32, void* hi, void* lo, int ld16, int dtype, int* err_flag, void* stream) {
   CHECK_CTX(c);

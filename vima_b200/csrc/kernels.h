@@ -130,5 +130,9 @@ cudaError_t launch_slot_kv_append(const unsigned short* qkv_hi, const unsigned s
                                   const int* q_pos, unsigned short* kv_hi, unsigned short* kv_lo, int ld_kv, int Lmax, cudaStream_t s);
 cudaError_t launch_slot_step_end(const float* x, int ldx, int S, int Q, int E, const unsigned char* step_mask, int* len, int* n_valid,
                                  int* has_action, const int* active, float* out, cudaStream_t s);
+cudaError_t launch_slot_kv_scatter(const unsigned short* qkv_hi, const unsigned short* qkv_lo, int ld_qkv, int col0, int width, int n, int Lq,
+                                   const int* slots, unsigned short* kv_hi, unsigned short* kv_lo, int ld_kv, int Lmax, cudaStream_t s);
+cudaError_t launch_slot_admit_prefix(const int* slots, int n, const unsigned char* prompt_mask, int Lp, int Lmax, unsigned char* slot_mask,
+                                     int* len, int* n_valid, int* has_action, int* active, cudaStream_t s);
 
 }  // namespace vima

@@ -119,4 +119,67 @@ cudaError_t launch_slot_step_end(const float* x, int ldx, int S, int Q, int E, c
   return cudaGetLastError();
 }
 
+// Admission of a decoder-only prompt (the prompt and its separator live in the self-attention cache, columns [0, Lq)).
+// Prefill rows (j, r) -> cache row slots[j]*Lmax + r, 8 16-bit values per thread and trip: each K/V element is read once and
+// written once.
+__global__ void slot_kv_scatter_kernel(const uint4* __restrict__ qkv_hi, const uint4* __restrict__ qkv_lo, int ld_qkv8, int col8, int w8, int n,
+                                       int Lq, const int* __restrict__ slots, uint4* __restrict__ kv_hi, uint4* __restrict__ kv_lo, int ld_kv8,
+                                       int Lmax) {
+  const long long total = (long long)n * Lq * w8;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % w8);
+    const long long jr = i / w8;
+    const int r = (int)(jr % Lq), j = (int)(jr / Lq);
+    const size_t src = (size_t)jr * ld_qkv8 + col8 + c;
+    const size_t dst = ((size_t)__ldg(slots + j) * Lmax + r) * ld_kv8 + c;
+    kv_hi[dst] = __ldg(qkv_hi + src);
+    if (kv_lo) kv_lo[dst] = __ldg(qkv_lo + src);
+  }
+}
+
+cudaError_t launch_slot_kv_scatter(const unsigned short* qkv_hi, const unsigned short* qkv_lo, int ld_qkv, int col0, int width, int n, int Lq,
+                                   const int* slots, unsigned short* kv_hi, unsigned short* kv_lo, int ld_kv, int Lmax, cudaStream_t s) {
+  const long long total = (long long)n * Lq * (width / 8);
+  if (total == 0) return cudaSuccess;
+  const int blocks = (int)min((total + 255) / 256, (long long)132 * 16);
+  slot_kv_scatter_kernel<<<blocks, 256, 0, s>>>(reinterpret_cast<const uint4*>(qkv_hi), reinterpret_cast<const uint4*>(qkv_lo), ld_qkv / 8,
+                                                col0 / 8, width / 8, n, Lq, slots, reinterpret_cast<uint4*>(kv_hi),
+                                                reinterpret_cast<uint4*>(kv_lo), ld_kv / 8, Lmax);
+  return cudaGetLastError();
+}
+
+// One block per admitted slot b = slots[j]: mask columns [0, Lp) <- prompt_mask[j], column Lp <- 1 (the separator); then
+// len = Lp+1, n_valid = valid prompt tokens + 1 (the separator's position id is the valid count), has_action = 0, active = 1.
+__global__ void __launch_bounds__(256) slot_admit_prefix_kernel(const int* __restrict__ slots, const unsigned char* __restrict__ prompt_mask,
+                                                                int Lp, int Lmax, unsigned char* __restrict__ slot_mask, int* __restrict__ len,
+                                                                int* __restrict__ n_valid, int* __restrict__ has_action,
+                                                                int* __restrict__ active) {
+  __shared__ int warp_cnt[8];
+  const int j = blockIdx.x, b = __ldg(slots + j);
+  int cnt = 0;
+  for (int l = threadIdx.x; l <= Lp; l += blockDim.x) {
+    const unsigned char m = l < Lp ? (prompt_mask[(size_t)j * Lp + l] != 0) : 1;
+    slot_mask[(size_t)b * Lmax + l] = m;
+    cnt += l < Lp ? m : 0;
+  }
+  cnt = __reduce_add_sync(0xffffffffu, cnt);
+  if ((threadIdx.x & 31) == 0) warp_cnt[threadIdx.x >> 5] = cnt;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int total = 0;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) total += warp_cnt[w];
+    len[b] = Lp + 1;
+    n_valid[b] = total + 1;
+    has_action[b] = 0;
+    active[b] = 1;
+  }
+}
+
+cudaError_t launch_slot_admit_prefix(const int* slots, int n, const unsigned char* prompt_mask, int Lp, int Lmax, unsigned char* slot_mask,
+                                     int* len, int* n_valid, int* has_action, int* active, cudaStream_t s) {
+  if (n == 0) return cudaSuccess;
+  slot_admit_prefix_kernel<<<n, 256, 0, s>>>(slots, prompt_mask, Lp, Lmax, slot_mask, len, n_valid, has_action, active);
+  return cudaGetLastError();
+}
+
 }  // namespace vima

@@ -80,20 +80,23 @@ class GraphedStep:
 
 
 class GraphedSlotStep:
-    """VIMAPolicy.step_slots for one (S, Q), captured into a CUDA graph.  The slot state (len / n_valid / has_action / active) lives
+    """A policy's step_slots for one (S, Q), captured into a CUDA graph.  The slot state (len / n_valid / has_action / active) lives
     on the device and the step's kernels read it, so admissions and releases between replays take effect.  Warm-up runs the step
     (which advances the slots), so the state vectors and their host mirror are snapshotted first and restored afterwards; the K/V and
     mask columns warm-up wrote lie at or past each slot's `len` and are never read before a step overwrites them.
 
         g = policy.capture_step_slots(cache, obs, obs_mask, action)   # cache state unchanged
         out = g(obs, obs_mask, action)                                # = policy.step_slots(cache, obs, obs_mask, action)
-    """
 
-    def __init__(self, policy, cache, obs_token: torch.Tensor, obs_mask: torch.Tensor, action_token: torch.Tensor, *, warmup: int = 2):
+    The step inputs are those of the policy's `_slot_step` after the cache: (obs_token, obs_mask, action_token) for VIMAPolicy,
+    (obs_token, action_token) for the baselines, whose obs tokens are all valid.  obs_token is (1,S,Q,E), or (1,S,E) with Q = 1."""
+
+    def __init__(self, policy, cache, obs_token: torch.Tensor, *inputs: torch.Tensor, warmup: int = 2):
         self.policy, self.cache = policy, cache
-        _, self.S, self.Q, self.E = obs_token.shape
+        self.S, self.E = obs_token.shape[1], obs_token.shape[-1]
+        self.Q = obs_token.shape[2] if obs_token.dim() == 4 else 1
         cache.check_step(self.S, self.Q, self.E, eng.prec())
-        self.static_in = [obs_token.clone(), obs_mask.clone(), action_token.float().clone()]
+        self.static_in = [obs_token.clone()] + [t.clone() for t in inputs[:-1]] + [inputs[-1].float().clone()]
         dev = obs_token.device
         self.ctx = _C.Context.get(dev)
         saved = cache.state()
@@ -115,11 +118,13 @@ class GraphedSlotStep:
             torch.cuda.synchronize(dev)
         self.replays = 0
 
-    def __call__(self, obs_token: torch.Tensor, obs_mask: torch.Tensor, action_token: torch.Tensor) -> torch.Tensor:
-        self.cache.check_step(obs_token.shape[1], obs_token.shape[2], obs_token.shape[3], eng.prec())
+    def __call__(self, obs_token: torch.Tensor, *inputs: torch.Tensor) -> torch.Tensor:
+        if len(inputs) + 1 != len(self.static_in):
+            raise ValueError(f"the graph was captured with {len(self.static_in)} step inputs, got {len(inputs) + 1}")
+        self.cache.check_step(obs_token.shape[1], obs_token.shape[2] if obs_token.dim() == 4 else 1, obs_token.shape[-1], eng.prec())
         if tuple(obs_token.shape) != tuple(self.static_in[0].shape):
             raise ValueError(f"the graph was captured for obs_token {tuple(self.static_in[0].shape)}, got {tuple(obs_token.shape)}")
-        for dst, src in zip(self.static_in, (obs_token, obs_mask, action_token)):
+        for dst, src in zip(self.static_in, (obs_token,) + inputs):
             if dst.data_ptr() != src.data_ptr():
                 dst.copy_(src, non_blocking=True)
         self.graph.replay()

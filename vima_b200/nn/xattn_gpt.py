@@ -104,15 +104,16 @@ class SlotDecodeCache:
     [S*Lp_cap, 2E]) with `prompt_mask` [S, Lp_cap] (a shorter prompt's tail columns are masked).  Per-slot device state, int32 [S]:
     `len` (cache columns used), `n_valid` (next position id), `has_action`, `active`; `q_pos` is the step's scratch copy of `len`.
     The host mirrors len / has_action / active (it knows them from admissions and the step width), so capacity is checked without
-    reading the device."""
+    reading the device.  A decoder-only model (HFGPT) opens it with Lp_cap = 0: its prompt and separator are the first columns of
+    the self-attention cache (HFGPT.prefill), and there is no prompt_kv / prompt_mask."""
 
     def __init__(self, *, S: int, Lmax: int, Lp_cap: int, E: int, n_layer: int, device, split: bool, precision: str):
         self.S, self.Lmax, self.Lp_cap, self.E, self.precision = S, Lmax, Lp_cap, E, precision
         mk = lambda rows: torch.zeros((rows, 2 * E), dtype=torch.int16, device=device)
         self.kv_hi = [mk(S * Lmax) for _ in range(n_layer)]
         self.kv_lo = [mk(S * Lmax) if split else None for _ in range(n_layer)]
-        self.prompt_kv = [eng.Opnd(S * Lp_cap, 2 * E, device, split, zero=True) for _ in range(n_layer)]
-        self.prompt_mask = torch.zeros((S, Lp_cap), dtype=torch.uint8, device=device)
+        self.prompt_kv = [eng.Opnd(S * Lp_cap, 2 * E, device, split, zero=True) for _ in range(n_layer)] if Lp_cap else None
+        self.prompt_mask = torch.zeros((S, Lp_cap), dtype=torch.uint8, device=device) if Lp_cap else None
         self.mask = torch.zeros((S, Lmax), dtype=torch.uint8, device=device)
         z = lambda: torch.zeros((S,), dtype=torch.int32, device=device)
         self.len, self.n_valid, self.has_action, self.active, self.q_pos = z(), z(), z(), z(), z()
@@ -170,11 +171,12 @@ def check_cache_append(cache: "DecodeCache", B: int, L: int, E: int, p) -> None:
 
 
 def run_block(ctx, p, W, blk: "Block", x32, x16, c16, *, B, L, E, H, omask, chain_ln=None, want16=False, out_f32=None, cache=None,
-              layer=0):
+              layer=0, kv_scatter=None):
     """GPT-1 post-LN block (components.py:23-37 / gpt.py:223-249): returns (LN2 output fp32, operands of the NEXT consumer):
     with `chain_ln` the operands are chain_ln(LN2(...)) (next layer's query LayerNorm), with `want16` they are LN2(...) itself.
     With `cache` (DecodeCache or SlotDecodeCache) the L rows are the NEW tokens of each episode and attention runs over the cached
-    prefix + themselves.
+    prefix + themselves.  With `kv_scatter` = (slots int32 [B], cache) and no `cache`, attention is local and the keys / values of
+    sequence j also go to rows slots[j]*Lmax + r of the cache (decoder-only prefill, HFGPT.prefill).
 
     ln_1 never runs as a kernel: c_proj's epilogue emits s = attn + x as fp32 + operands together with per-row partial sums, the
     GEGLU GEMM takes the un-normalised s with ln_1 folded into its weights (rstd / mean applied in its epilogue), and the MLP's
@@ -187,6 +189,9 @@ def run_block(ctx, p, W, blk: "Block", x32, x16, c16, *, B, L, E, H, omask, chai
     _, qkv16 = eng.gemm(ctx, x16, W["c_attn"], p, want16=True)
     o8 = None if c16.lo8 is None else (c16.lo8, c16.hi8)
     if cache is None:
+        if kv_scatter is not None:
+            sl, kc = kv_scatter
+            ctx.slot_kv_scatter(qkv16.hi, qkv16.lo, qkv16.ld, E, 2 * E, B, L, sl, kc.kv_hi[layer], kc.kv_lo[layer], 2 * E, kc.Lmax)
         ctx.attention(q=(qkv16.hi, qkv16.lo, qkv16.ld, 0), k=(qkv16.hi, qkv16.lo, qkv16.ld, E), v=(qkv16.hi, qkv16.lo, qkv16.ld, 2 * E),
                       o=(c16.hi, c16.lo, c16.ld, 0), B=B, H=H, Lq=L, Lk=L, D=d, scale=1.0 / math.sqrt(d), causal=True, key_mask=omask,
                       dtype=p.dtype, o8=o8)
@@ -560,8 +565,11 @@ class HFGPT(nn.Module):
             del state_dict[k]
 
     def forward(self, x: torch.Tensor, *, custom_mask: Optional[torch.Tensor] = None, position_ids: Optional[torch.Tensor] = None,
-                batch_first: bool = False):
-        """x: (L,B,E) if not batch_first else (B,L,E); custom_mask (B,L) or (B,1,L) combined with the causal mask (gpt.py:46-79)."""
+                batch_first: bool = False, cache=None):
+        """x: (L,B,E) if not batch_first else (B,L,E); custom_mask (B,L) or (B,1,L) combined with the causal mask (gpt.py:46-79).
+        With `cache` (DecodeCache or SlotDecodeCache, opened by `prefill`) x, custom_mask and absolute position_ids describe only the
+        tokens appended this step and only their rows are returned: a DecodeCache takes their mask columns and advances `L`; for a
+        SlotDecodeCache x is one step block per slot as vima_slot_step_begin lays it out (it has written the mask columns)."""
         ctx = eng.ctx_for(x)
         p = eng.prec()
         if batch_first:
@@ -569,6 +577,54 @@ class HFGPT(nn.Module):
         else:
             L, B, E = x.shape
         assert E == self.n_embd and L <= self.n_positions
+        slots = isinstance(cache, SlotDecodeCache)
+        if cache is not None:
+            if position_ids is None or custom_mask is None:
+                raise ValueError("cached decode needs absolute position ids and masks for the appended tokens")
+            if slots:
+                cache.check_step(B, L - 1, E, p)
+            else:
+                check_cache_append(cache, B, L, E, p)
+        omask = None
+        if custom_mask is not None:
+            if custom_mask.dim() == 3:
+                custom_mask = custom_mask.squeeze(dim=1)
+            omask = eng.as_u8(custom_mask != 0)
+        if cache is not None and not slots:
+            cache.mask[:, cache.L:cache.L + L].copy_(omask)
+        out = self._stack(ctx, p, x, omask, position_ids, batch_first, cache=cache)
+        if cache is not None and not slots:
+            cache.L += L
+        return out
+
+    @torch.no_grad()
+    def prefill(self, cache, slots: list, x: torch.Tensor, custom_mask_u8: torch.Tensor, position_ids: torch.Tensor) -> None:
+        """Decoder-only prompt prefill.  x (L,n,E) holds n new sequences [prompt | separator] (custom_mask_u8 / position_ids (n,L);
+        the separator, last, is valid).  They run through every block with local causal attention -- the arithmetic of `forward` --
+        and after each layer's c_attn GEMM their keys / values go to cache rows slots[j]*Lmax + r (vima_slot_kv_scatter).  Then the
+        mask columns [0, L) and the state are set: a SlotDecodeCache's by vima_slot_admit_prefix (len = L, n_valid = valid tokens,
+        no action, active), a DecodeCache's (slots = all its rows, in order) by copying the mask and setting L and n_valid.  The
+        caller has validated shapes, slots, capacity and the precision mode."""
+        ctx = eng.ctx_for(x)
+        p = eng.prec()
+        L, n, E = x.shape
+        sl = torch.tensor(slots, dtype=torch.int32, device=x.device)
+        self._stack(ctx, p, x, custom_mask_u8, position_ids, False, kv_scatter=(sl, cache))
+        if isinstance(cache, SlotDecodeCache):
+            ctx.slot_admit_prefix(sl, custom_mask_u8[:, :L - 1].contiguous(), cache.Lmax, cache.mask, len_=cache.len, n_valid=cache.n_valid,
+                                  has_action=cache.has_action, active=cache.active)
+            for b in slots:
+                cache.len_host[b], cache.has_action_host[b], cache.active_host[b] = L, False, True
+        else:
+            cache.mask[:, :L].copy_(custom_mask_u8)
+            cache.n_valid.copy_(custom_mask_u8.sum(dim=1))
+            cache.L = L
+
+    def _stack(self, ctx, p, x, omask, position_ids, batch_first, *, cache=None, kv_scatter=None):
+        if batch_first:
+            B, L, E = x.shape
+        else:
+            L, B, E = x.shape
         dev = x.device
         xf = x.float()
         if xf.stride(-1) != 1:
@@ -577,11 +633,6 @@ class HFGPT(nn.Module):
         if position_ids is None:
             position_ids = self.lm.position_ids[None, :L].expand(B, L)
         ids = position_ids.to(torch.int64).contiguous()
-        omask = None
-        if custom_mask is not None:
-            if custom_mask.dim() == 3:
-                custom_mask = custom_mask.squeeze(dim=1)
-            omask = eng.as_u8(custom_mask != 0)
         M, H = B * L, self.n_head
         x32 = torch.empty((M, E), dtype=torch.float32, device=dev)
         x16 = eng.Opnd(M, E, dev, p.split, f8=p.f8)
@@ -591,6 +642,7 @@ class HFGPT(nn.Module):
         layers = self._wc.get("blocks", tuple(self.lm.h.parameters()), lambda: [pack_block(ctx, blk, p) for blk in self.lm.h])
         c16 = eng.Opnd(M, E, dev, p.split, f8=p.f8)
         for i, (blk, W) in enumerate(zip(self.lm.h, layers)):
-            x32, x16 = run_block(ctx, p, W, blk, x32, x16, c16, B=B, L=L, E=E, H=H, omask=omask, want16=i + 1 < self.n_layer)
+            x32, x16 = run_block(ctx, p, W, blk, x32, x16, c16, B=B, L=L, E=E, H=H, omask=omask, want16=i + 1 < self.n_layer, cache=cache,
+                                 layer=i, kv_scatter=kv_scatter)
         out = x32.view(B, L, E)
         return out if batch_first else out.transpose(0, 1)

@@ -16,6 +16,7 @@ from .. import engine as eng
 from .. import nn as vnn
 from ..utils import *  # noqa: F401,F403
 from .vima_gato_policy import VIMAGatoPolicy
+from .vima_policy import VIMAPolicy
 
 
 class VIMAFlamingoPolicy(VIMAGatoPolicy):
@@ -77,6 +78,51 @@ class VIMAFlamingoPolicy(VIMAGatoPolicy):
                              scratch_m, scratch_p)
         out = self.xattn_gpt(obs_action_tokens=tokens, prompt_tokens=prompt_token, prompt_mask=prompt_token_mask)
         return out[Q - 1 :: Q + 1]
+
+    # --------------------------------------------------------------------------------------------------
+    # Cached and slot decode: VIMAPolicy's (the same XAttnGPT decoder) with the two differences of `forward` above: every obs token
+    # is valid, and the prompt position ids are the default arange.  Every decode method is defined here, so none of VIMA-Gato's
+    # decoder-only versions is inherited.
+    def _prompt_positions(self, ctx, pmask_u8: torch.Tensor) -> torch.Tensor:
+        n, Lp = pmask_u8.shape
+        return self.xattn_gpt.xattn_position_ids[None, :Lp].expand(n, Lp).contiguous()
+
+    def _ones(self, obs_token: torch.Tensor) -> torch.Tensor:
+        return torch.ones(obs_token.shape[:3], dtype=torch.bool, device=obs_token.device)
+
+    def start_decode(self, prompt_token: torch.Tensor, prompt_token_mask: torch.Tensor, *, max_tokens: Optional[int] = None):
+        """prompt_token (Lp,B,E), prompt_token_mask (B,Lp); room for `max_tokens` history tokens (default: n_positions)."""
+        return VIMAPolicy.start_decode(self, prompt_token, prompt_token_mask, max_tokens=max_tokens)
+
+    def forward_step(self, cache, obs_token: torch.Tensor, prev_action_token: Optional[torch.Tensor]):
+        """obs_token (1,B,Q,E), prev_action_token (1,B,E) (None at the first step) -> (1,B,E); equals `forward(...)[-1:]`."""
+        eng.ctx_for(obs_token)
+        self._check_obs(obs_token.shape[2])
+        return VIMAPolicy.forward_step(self, cache, obs_token, self._ones(obs_token), prev_action_token)
+
+    def open_slots(self, n_slots: int, *, max_tokens: Optional[int] = None, max_prompt_tokens: int = 256):
+        return VIMAPolicy.open_slots(self, n_slots, max_tokens=max_tokens, max_prompt_tokens=max_prompt_tokens)
+
+    def admit(self, cache, slots, prompt_token: torch.Tensor, prompt_token_mask: torch.Tensor) -> None:
+        eng.ctx_for(prompt_token)
+        return VIMAPolicy.admit(self, cache, slots, prompt_token, prompt_token_mask)
+
+    release = VIMAPolicy.release
+
+    def step_slots(self, cache, obs_token: torch.Tensor, action_token: Optional[torch.Tensor]) -> torch.Tensor:
+        """obs_token (1,S,Q,E), action_token (1,S,E) | None -> (1,S,E), as VIMAPolicy.step_slots with every obs token valid."""
+        # the checks and host bookkeeping shared with VIMA-Gato; the device step is this class's _slot_step
+        return VIMAGatoPolicy.step_slots(self, cache, obs_token, action_token)
+
+    def _slot_step(self, cache, obs_token, action_token):
+        return VIMAPolicy._slot_step(self, cache, obs_token, self._ones(obs_token), action_token)
+
+    def capture_step_slots(self, cache, obs_token: torch.Tensor, action_token: torch.Tensor, *, warmup: int = 2):
+        """`step_slots` captured into one CUDA graph; call the result as g(obs_token, action_token)."""
+        from ..graphs import GraphedSlotStep
+
+        self._check_obs(obs_token.shape[2])
+        return GraphedSlotStep(self, cache, obs_token, action_token, warmup=warmup)
 
     # forward_prompt_assembly (:165-228) and forward_obs_token (:230-240) are the inherited token-per-query versions with
     # `_obj_xf_num_queries == 4`: the object encoder returns (n, 4, E).

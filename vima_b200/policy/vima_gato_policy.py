@@ -89,6 +89,148 @@ class VIMAGatoPolicy(nn.Module):
         tokens_out = self.transformer(tokens, custom_mask=mask.view(torch.bool), batch_first=False, position_ids=position_ids)
         return tokens_out[Lp + 1 + Q - 1 :: Q + 1]
 
+    # --------------------------------------------------------------------------------------------------
+    # Cached decode (DESIGN.md 7 (f)1; not in the reference, which re-runs [prompt | separator | history] every step).  The prompt
+    # and separator are prefilled once into the first Lp+1 columns of the self-attention cache; a step appends [a_{t-1}, o_t^1..Q].
+    def _prompt_prefix(self, ctx, prompt_token: torch.Tensor, prompt_token_mask: torch.Tensor):
+        """[prompt | separator] tokens (Lp+1,n,E), mask (n,Lp+1) uint8 and position ids (n,Lp+1): the first Lp+1 rows of `forward`."""
+        Lp, n, E = prompt_token.shape
+        dev = prompt_token.device
+        tokens = torch.empty((Lp + 1, n, E), dtype=torch.float32, device=dev)
+        tokens[:Lp].copy_(prompt_token)
+        tokens[Lp].copy_(self.prompt_sep_token.detach().unsqueeze(0).expand(n, E))
+        mask = torch.empty((n, Lp + 1), dtype=torch.uint8, device=dev)
+        pos = torch.empty((n, Lp + 1), dtype=torch.int64, device=dev)
+        ctx.gato_positions(eng.as_u8(prompt_token_mask).contiguous(), Lp + 1, mask, pos)
+        return tokens, mask, pos
+
+    def _check_prompt(self, prompt_token: torch.Tensor, prompt_token_mask: torch.Tensor, n: int, Lmax: int) -> None:
+        Lp, nb, E = prompt_token.shape
+        if nb != n or E != self.embed_dim or tuple(prompt_token_mask.shape) != (n, Lp):
+            raise ValueError(f"expected prompt_token (Lp, {n}, {self.embed_dim}) and a ({n}, Lp) mask, got {tuple(prompt_token.shape)} / "
+                             f"{tuple(prompt_token_mask.shape)}")
+        if Lp + 1 >= Lmax:
+            raise ValueError(f"a prompt of {Lp} tokens + separator leaves no room in max_tokens={Lmax}")
+
+    def _check_obs(self, Q: int) -> None:
+        if Q != self._obj_xf_num_queries:
+            raise ValueError(f"an observation is {self._obj_xf_num_queries} tokens, got {Q}")
+
+    def start_decode(self, prompt_token: torch.Tensor, prompt_token_mask: torch.Tensor, *, max_tokens: Optional[int] = None):
+        """Open a K/V cache for a batch of episodes and prefill [prompt | separator]: prompt_token (Lp,B,E), prompt_token_mask
+        (B,Lp); `max_tokens` columns per episode, prompt and separator included (default: the decoder's n_positions, which bounds
+        the whole sequence).  Feed it to `forward_step` once per environment step."""
+        ctx = eng.ctx_for(prompt_token)
+        Lp, B, E = prompt_token.shape
+        n_pos = self.transformer.n_positions
+        Lmax = n_pos if max_tokens is None else int(max_tokens)
+        if Lmax > n_pos:
+            raise ValueError(f"max_tokens={Lmax} exceeds n_positions={n_pos}")
+        self._check_prompt(prompt_token, prompt_token_mask, B, Lmax)
+        p = eng.prec()
+        cache = vnn.DecodeCache(B=B, Lmax=Lmax, E=E, n_layer=self.transformer.n_layer, device=prompt_token.device, split=p.split,
+                                precision=p.name)
+        cache.prefix = Lp + 1  # columns before the first step
+        self.transformer.prefill(cache, list(range(B)), *self._prompt_prefix(ctx, prompt_token, prompt_token_mask))
+        return cache
+
+    def forward_step(self, cache, obs_token: torch.Tensor, prev_action_token: Optional[torch.Tensor]):
+        """One environment step through the cache: obs_token (1,B,Q,E), prev_action_token (1,B,E) (None at the first step) ->
+        predicted action token (1,B,E); equals `forward(...)[-1:]` over the whole history.  Every history token is valid, so the
+        step's position ids are n_valid + arange (vima_gato_policy.py:172-183)."""
+        ctx = eng.ctx_for(obs_token)
+        _, B, Q, E = obs_token.shape
+        self._check_obs(Q)
+        if (prev_action_token is None) != (cache.L == cache.prefix):
+            raise ValueError("forward_step: exactly one action token per previous step is required")
+        L = Q + (0 if prev_action_token is None else 1)
+        from ..nn.xattn_gpt import check_cache_append
+
+        check_cache_append(cache, B, L, E, eng.prec())  # every refusal happens before the cache is touched
+        new = obs_token[0].float()
+        if prev_action_token is not None:
+            new = torch.cat([prev_action_token[0].float().unsqueeze(1), new], dim=1)
+        new = new.contiguous()
+        dev = obs_token.device
+        pos = cache.n_valid[:, None] + torch.arange(L, dtype=torch.int64, device=dev)[None, :]
+        ones = torch.ones((B, L), dtype=torch.bool, device=dev)
+        out = self.transformer(new, custom_mask=ones, position_ids=pos, batch_first=True, cache=cache)
+        cache.n_valid += L
+        return out[:, -1:].transpose(0, 1)
+
+    # Slot decode: each row of the batch holds one episode at its own length (VIMAPolicy.open_slots ... capture_step_slots).  A
+    # slot's columns [0, Lp+1) hold its prompt and separator; the step kernels are VIMAPolicy's with an all-ones obs mask, so their
+    # position rule n_valid + cumsum - 1 is Gato's n_valid + arange.
+    def open_slots(self, n_slots: int, *, max_tokens: Optional[int] = None):
+        """Allocate a SlotDecodeCache of `n_slots` slots (all inactive) of `max_tokens` columns each, prompt and separator included
+        (default: the decoder's n_positions), in the current precision mode."""
+        w = self.transformer.lm.positions_embed.weight
+        eng.ctx_for(w)
+        n_pos = self.transformer.n_positions
+        Lmax = n_pos if max_tokens is None else int(max_tokens)
+        if not 2 < Lmax <= n_pos:
+            raise ValueError(f"max_tokens={Lmax} outside (2, n_positions={n_pos}]")
+        if n_slots < 1:
+            raise ValueError("n_slots must be >= 1")
+        p = eng.prec()
+        return vnn.SlotDecodeCache(S=int(n_slots), Lmax=Lmax, Lp_cap=0, E=self.embed_dim, n_layer=self.transformer.n_layer, device=w.device,
+                                   split=p.split, precision=p.name)
+
+    def admit(self, cache, slots, prompt_token: torch.Tensor, prompt_token_mask: torch.Tensor) -> None:
+        """Start a new episode in each of `slots` (replacing whatever they held): prompt_token (Lp,n,E), prompt_token_mask (n,Lp).
+        Prefills the n new [prompt | separator] sequences only, on the current stream."""
+        ctx = eng.ctx_for(prompt_token)
+        s = cache.slot_index(slots)
+        if cache.prompt_kv is not None:
+            raise ValueError("admit: this SlotDecodeCache was opened for a cross-attention decoder")
+        self._check_prompt(prompt_token, prompt_token_mask, len(s), cache.Lmax)
+        cache.check_precision(eng.prec())
+        if not s:
+            return
+        self.transformer.prefill(cache, s, *self._prompt_prefix(ctx, prompt_token, prompt_token_mask))
+
+    release = VIMAPolicy.release
+
+    def step_slots(self, cache, obs_token: torch.Tensor, action_token: Optional[torch.Tensor]) -> torch.Tensor:
+        """One environment step of every slot: obs_token (1,S,Q,E), action_token (1,S,E) (each slot's previous action; ignored for
+        slots at their first step; None = all zeros) -> predicted action token (1,S,E).  For an active slot the row equals
+        `forward(...)[-1:]` at B=1 over that episode's own history; an inactive slot's row is unspecified."""
+        eng.ctx_for(obs_token)
+        _, S, Q, E = obs_token.shape
+        self._check_obs(Q)
+        cache.check_step(S, Q, E, eng.prec())
+        out = self._slot_step(cache, obs_token, action_token)
+        cache.advance_host(Q)
+        return out
+
+    def _slot_step(self, cache, obs_token, action_token):
+        """The device side of `step_slots` (static shapes, no host synchronisation; captured by GraphedSlotStep)."""
+        ctx = eng.ctx_for(obs_token)
+        _, S, Q, E = obs_token.shape
+        dev = obs_token.device
+        L = Q + 1
+        obs = obs_token[0].float().contiguous()
+        ones = torch.ones((S, Q), dtype=torch.uint8, device=dev)
+        act = torch.zeros((S, E), dtype=torch.float32, device=dev) if action_token is None else action_token[0].float().contiguous()
+        tokens = torch.empty((S * L, E), dtype=torch.float32, device=dev)
+        step_mask = torch.empty((S, L), dtype=torch.uint8, device=dev)
+        pos = torch.empty((S, L), dtype=torch.int64, device=dev)
+        ctx.slot_step_begin(obs, ones, act, Lmax=cache.Lmax, len_=cache.len, n_valid=cache.n_valid, has_action=cache.has_action,
+                            active=cache.active, tokens=tokens, step_mask=step_mask, pos=pos, q_pos=cache.q_pos, slot_mask=cache.mask)
+        x = self.transformer(tokens.view(S, L, E), custom_mask=step_mask.view(torch.bool), position_ids=pos, batch_first=True, cache=cache)
+        out = torch.empty((S, E), dtype=torch.float32, device=dev)
+        ctx.slot_step_end(x.reshape(S * L, E), S, Q, E, step_mask, len_=cache.len, n_valid=cache.n_valid, has_action=cache.has_action,
+                          active=cache.active, out=out)
+        return out.view(1, S, E)
+
+    def capture_step_slots(self, cache, obs_token: torch.Tensor, action_token: torch.Tensor, *, warmup: int = 2):
+        """`step_slots` for this (S, Q) captured into one CUDA graph (vima_b200.graphs.GraphedSlotStep); the cache's slot state is
+        left as it was.  Call the result like step_slots without the cache: g(obs_token, action_token)."""
+        from ..graphs import GraphedSlotStep
+
+        self._check_obs(1 if obs_token.dim() == 3 else obs_token.shape[2])
+        return GraphedSlotStep(self, cache, obs_token, action_token, warmup=warmup)
+
     def forward_prompt_assembly(self, prompts):
         """(token_types, word_batch, image_batch{"rgb": {view: (n_img,3,64,128)}}) -> (Lp,B,E), (B,Lp) bool (:193-251)."""
         raw_prompts_token_type, word_batch, image_batch = prompts

@@ -64,6 +64,20 @@ class VIMAGPTPolicy(VIMAGatoPolicy):
         (vima_gpt_policy.py:119-176): the Gato layout with one token per observation."""
         return VIMAGatoPolicy.forward(self, obs_token.unsqueeze(2), action_token, prompt_token, prompt_token_mask)
 
+    # Cached and slot decode: VIMA-Gato's with one token per observation.  start_decode, open_slots, admit, release and
+    # capture_step_slots are the inherited ones (capture takes obs_token (1,S,E)).
+    def forward_step(self, cache, obs_token: torch.Tensor, prev_action_token: Optional[torch.Tensor]):
+        """obs_token (1,B,E), prev_action_token (1,B,E) (None at the first step) -> (1,B,E)."""
+        return VIMAGatoPolicy.forward_step(self, cache, obs_token.unsqueeze(2), prev_action_token)
+
+    def step_slots(self, cache, obs_token: torch.Tensor, action_token: Optional[torch.Tensor]) -> torch.Tensor:
+        """obs_token (1,S,E), action_token (1,S,E) | None -> (1,S,E)."""
+        return VIMAGatoPolicy.step_slots(self, cache, obs_token.unsqueeze(2), action_token)
+
+    def _slot_step(self, cache, obs_token, action_token):
+        """obs_token (1,S,E) from a captured graph's inputs, or (1,S,1,E) from step_slots."""
+        return VIMAGatoPolicy._slot_step(self, cache, obs_token.unsqueeze(2) if obs_token.dim() == 3 else obs_token, action_token)
+
     # forward_prompt_assembly (vima_gpt_policy.py:178-238) is the inherited one with `_obj_xf_num_queries == 1`: the image
     # encoder returns (n_img, 2E), the post-MLP (n_img, 768), one prompt slot per image.
 

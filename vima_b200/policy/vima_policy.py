@@ -99,9 +99,14 @@ class VIMAPolicy(nn.Module):
         cache = vnn.DecodeCache(B=B, Lmax=Lmax, E=E, n_layer=self.xattn_gpt.n_layer, device=prompt_token.device, split=eng.prec().split,
                                 precision=eng.prec().name)
         pmask_u8 = eng.as_u8(prompt_token_mask)
-        cache.prompt = (prompt_token, pmask_u8, torch.empty(pmask_u8.shape, dtype=torch.int64, device=prompt_token.device))
-        ctx.mask_cumsum(pmask_u8, cache.prompt[2])
+        cache.prompt = (prompt_token, pmask_u8, self._prompt_positions(ctx, pmask_u8))
         return cache
+
+    def _prompt_positions(self, ctx, pmask_u8: torch.Tensor) -> torch.Tensor:
+        """Prompt position ids of the cached paths: cumsum(mask) - 1, as `forward` computes them (vima_policy.py:147)."""
+        pos = torch.empty(pmask_u8.shape, dtype=torch.int64, device=pmask_u8.device)
+        ctx.mask_cumsum(pmask_u8, pos)
+        return pos
 
     def forward_step(self, cache, obs_token: torch.Tensor, obs_mask: torch.Tensor, prev_action_token: Optional[torch.Tensor]):
         """One environment step through the cache: obs_token (1,B,Q,E), obs_mask (1,B,Q), prev_action_token (1,B,E) (None at
@@ -168,9 +173,7 @@ class VIMAPolicy(nn.Module):
             return
         ctx = eng.ctx_for(prompt_token)
         pmask_u8 = eng.as_u8(prompt_token_mask)
-        prompt_pos = torch.empty(pmask_u8.shape, dtype=torch.int64, device=prompt_token.device)
-        ctx.mask_cumsum(pmask_u8, prompt_pos)
-        self.xattn_gpt.admit_prompts(cache, s, prompt_token, pmask_u8, prompt_pos)
+        self.xattn_gpt.admit_prompts(cache, s, prompt_token, pmask_u8, self._prompt_positions(ctx, pmask_u8))
 
     def release(self, cache, slots) -> None:
         """Mark `slots` inactive (their episodes ended); they keep computing on whatever is passed but never advance."""
