@@ -28,31 +28,17 @@ struct Op16<DT_F16> {
   using T = __half;
   static __device__ __forceinline__ unsigned short bits(float x) { return __half_as_ushort(__float2half_rn(x)); }
   static __device__ __forceinline__ float back(unsigned short b) { return __half2float(__ushort_as_half(b)); }
-  static __device__ __forceinline__ unsigned short bits_sat(float x) {
-    x = fminf(fmaxf(x, -65504.f), 65504.f);
-    return bits(x);
-  }
 };
 template <>
 struct Op16<DT_BF16> {
   using T = __nv_bfloat16;
   static __device__ __forceinline__ unsigned short bits(float x) { return __bfloat16_as_ushort(__float2bfloat16_rn(x)); }
   static __device__ __forceinline__ float back(unsigned short b) { return __bfloat162float(__ushort_as_bfloat16(b)); }
-  static __device__ __forceinline__ unsigned short bits_sat(float x) { return bits(x); }
 };
-
-template <int DT>
-__device__ __forceinline__ void split16(float x, unsigned short& hi, unsigned short& lo) {
-  hi = Op16<DT>::bits_sat(x);
-  lo = Op16<DT>::bits(x - Op16<DT>::back(hi));
-}
-
-__device__ __forceinline__ void split16_rt(int dt, float x, unsigned short& hi, unsigned short& lo) {
-  if (dt == DT_F16) split16<DT_F16>(x, hi, lo); else split16<DT_BF16>(x, hi, lo);
-}
 
 // Packed pair split: two F2FP (saturating, so |x| > 65504 degrades instead of producing inf/NaN) + one unpack.
 // Low 16 bits = first element.  3 instructions per element instead of 7 for the scalar form.
+// Both halves saturate: +-inf -> +-MAX_NORM in hi and lo, NaN -> NaN in hi and lo.
 template <int DT>
 __device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_t& lo) {
   if constexpr (DT == DT_F16) {
@@ -64,6 +50,16 @@ __device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_
     const float2 hf = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&hi));
     asm("cvt.rn.satfinite.bf16x2.f32 %0, %1, %2;" : "=r"(lo) : "f"(x1 - hf.y), "f"(x0 - hf.x));
   }
+}
+
+// Scalar split (module inputs, weight packing): the packed form on (x, 0), so every producer of an operand pair gives the
+// same bits for the same value, including |x| > 65504, +-inf and NaN.
+template <int DT>
+__device__ __forceinline__ void split16(float x, unsigned short& hi, unsigned short& lo) {
+  uint32_t h2, l2;
+  split2<DT>(x, 0.f, h2, l2);
+  hi = (unsigned short)(h2 & 0xFFFFu);
+  lo = (unsigned short)(l2 & 0xFFFFu);
 }
 // ---- fp8 (e4m3) cross-term operands ("f16f8" mode, DESIGN.md section 3) --------------------------------------------
 // a*b ~= a_hi16*b_hi16 + a_lo8*b_hi8 + a_hi8*b_lo8 with   a_lo8 = e4m3((a - a_hi16) * 2^10),  a_hi8 = e4m3(a * 2^-3),
