@@ -287,8 +287,6 @@ int vima_gemm(vima_ctx* c, const vima_gemm_desc* d_in, void* stream) {
     if ((rc = make_tmap_f8(c, &p.tm_b_lo, d->b_lo8, d->N, d->K, d->ldb8, bn))) return rc;
   }
   p.M = d->M; p.N = d->N; p.K = d->K;
-  p.block_n = bn;
-  p.split = split;
   p.dtype = d->dtype;
   p.glu = d->glu;
   p.epi_prefetch = c->epi_prefetch;
@@ -317,8 +315,11 @@ int vima_gemm(vima_ctx* c, const vima_gemm_desc* d_in, void* stream) {
   l.act = d->act; l.glu = d->glu != 0; l.mul = d->mul != nullptr; l.res = d->residual != nullptr;
   l.o32 = d->out_f32 != nullptr; l.o16 = d->out_hi != nullptr; l.dtype = d->dtype;
   l.lna = d->row_stats != nullptr; l.lnr = d->res_stats != nullptr; l.stats = d->stats_out != nullptr; l.device = c->device;
-  if (d->dtype == DT_BF16) { LAUNCHED(c, launch_gemm_tc_bf16(p, l, grid, smem, c->max_smem_optin, (cudaStream_t)stream), "gemm_tc_kernel"); }
-  LAUNCHED(c, launch_gemm_tc_f16(p, l, grid, smem, c->max_smem_optin, (cudaStream_t)stream), "gemm_tc_kernel");
+  l.split = split; l.block_n = bn;
+  // f16f8 (split 2) is fp16-only (checked above)
+  auto launch = d->dtype == DT_BF16 ? (split ? launch_gemm_tc<DT_BF16, 1> : launch_gemm_tc<DT_BF16, 0>)
+                                    : (split == 2 ? launch_gemm_tc<DT_F16, 2> : split ? launch_gemm_tc<DT_F16, 1> : launch_gemm_tc<DT_F16, 0>);
+  LAUNCHED(c, launch(p, l, grid, smem, c->max_smem_optin, (cudaStream_t)stream), "gemm_tc_kernel");
 }
 
 int vima_gemm_f32_grouped(vima_ctx* c, const vima_f32_gemm_group* groups_dev, int n_groups, int M, int max_n, int act, void* stream) {

@@ -156,11 +156,11 @@ __global__ void __launch_bounds__(ATC_THREADS, 2) attention_tc_kernel(const __gr
         const uint64_t dkh = wgmma_desc_sw64(sbase + OFF_K + stage * 8192), dkl = wgmma_desc_sw64(sbase + OFF_K + stage * 8192 + 4096);
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < ATC_D / 16; ++k) wgmma_m64n64k16_ss<DT>(s, dqh + 2 * k, dkh + 2 * k, (uint32_t)(k != 0));
+        for (int k = 0; k < ATC_D / 16; ++k) wgmma_m64nNk16_ss<DT, 64>(s, dqh + 2 * k, dkh + 2 * k, (uint32_t)(k != 0));
 #pragma unroll
-        for (int k = 0; k < ATC_D / 16; ++k) wgmma_m64n64k16_ss<DT>(s, dql + 2 * k, dkh + 2 * k, 1u);
+        for (int k = 0; k < ATC_D / 16; ++k) wgmma_m64nNk16_ss<DT, 64>(s, dql + 2 * k, dkh + 2 * k, 1u);
 #pragma unroll
-        for (int k = 0; k < ATC_D / 16; ++k) wgmma_m64n64k16_ss<DT>(s, dqh + 2 * k, dkl + 2 * k, 1u);
+        for (int k = 0; k < ATC_D / 16; ++k) wgmma_m64nNk16_ss<DT, 64>(s, dqh + 2 * k, dkl + 2 * k, 1u);
         wgmma_commit();
       }
       // V(c) -> V^T tile (dim n, key k at n*128 + (((k>>3) ^ (n&7)) << 4) + (k&7)*2), while the tensor cores work on S

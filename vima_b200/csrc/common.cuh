@@ -170,17 +170,14 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a protocol bug traps instead of hanging the GPU box.
+// Bounded wait: a protocol bug traps (the launch fails with an error) instead of hanging the GPU.  No printf on the timeout
+// path: a function call inside a wgmma loop makes ptxas serialise every wgmma of the kernel.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if ((++spins & 1023u) == 0u && clock64() - t0 > VIMA_WAIT_CYCLES) {
-      printf("vima_b200: mbarrier timeout block (%d,%d,%d) thread %d bar %u parity %u\n", (int)blockIdx.x, (int)blockIdx.y, (int)blockIdx.z,
-             (int)threadIdx.x, smem_u32(bar), parity);
-      __trap();
-    }
+    if ((++spins & 1023u) == 0u && clock64() - t0 > VIMA_WAIT_CYCLES) __trap();
   }
 }
 
@@ -220,36 +217,59 @@ __device__ __forceinline__ void wgmma_fence_acc(float (&d)[N]) {  // keeps the c
   for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-#define VIMA_ACC32(d)                                                                                                        \
-  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), \
-      "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),  \
-      "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), \
-      "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-#define VIMA_ACC16(d)                                                                                                        \
-  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), \
-      "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+#define VIMA_ACC8(d, o)                                                                                                  \
+  "+f"(d[(o) + 0]), "+f"(d[(o) + 1]), "+f"(d[(o) + 2]), "+f"(d[(o) + 3]), "+f"(d[(o) + 4]), "+f"(d[(o) + 5]), "+f"(d[(o) + 6]), \
+      "+f"(d[(o) + 7])
+#define VIMA_ACC16(d) VIMA_ACC8(d, 0), VIMA_ACC8(d, 8)
+#define VIMA_ACC32(d) VIMA_ACC16(d), VIMA_ACC8(d, 16), VIMA_ACC8(d, 24)
+#define VIMA_ACC48(d) VIMA_ACC32(d), VIMA_ACC8(d, 32), VIMA_ACC8(d, 40)
+#define VIMA_ACC64(d) VIMA_ACC48(d), VIMA_ACC8(d, 48), VIMA_ACC8(d, 56)
+#define VIMA_R16 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}"
 #define VIMA_R32 \
   "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}"
-#define VIMA_R16 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}"
+#define VIMA_R48 \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}"
+#define VIMA_R64 \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}"
 
-// 16-bit operands (DT_F16 / DT_BF16), both K-major in shared memory: M64 N64 K16
-template <int DT>
-__device__ __forceinline__ void wgmma_m64n64k16_ss(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
-  if constexpr (DT == DT_F16) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 " VIMA_R32 ", %32, %33, p, 1, 1, 0, 0;\n\t}"
-                 : VIMA_ACC32(d) : "l"(da), "l"(db), "r"(accumulate));
-  } else {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " VIMA_R32 ", %32, %33, p, 1, 1, 0, 0;\n\t}"
-                 : VIMA_ACC32(d) : "l"(da), "l"(db), "r"(accumulate));
-  }
+// 16-bit operands (DT_F16 / DT_BF16), both K-major in shared memory: M64 N{N} K16.  IA / IB / IP: operand numbers of the A and
+// B descriptors and of the scale-d flag (they follow the N/2 accumulator operands).
+#define VIMA_WGMMA_K16(N, R, ACC, IA, IB, IP)                                                                                      \
+  if constexpr (DT == DT_F16)                                                                                                      \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, " IP ", 0;\n\t"                                                             \
+                 "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32.f16.f16 " R ", " IA ", " IB ", p, 1, 1, 0, 0;\n\t}"              \
+                 : ACC(d) : "l"(da), "l"(db), "r"(accumulate));                                                                    \
+  else                                                                                                                             \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, " IP ", 0;\n\t"                                                             \
+                 "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32.bf16.bf16 " R ", " IA ", " IB ", p, 1, 1, 0, 0;\n\t}"            \
+                 : ACC(d) : "l"(da), "l"(db), "r"(accumulate))
+template <int DT, int N>
+__device__ __forceinline__ void wgmma_m64nNk16_ss(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
+  static_assert(N == 32 || N == 64 || N == 96 || N == 128, "wgmma_m64nNk16_ss: N is 32, 64, 96 or 128");
+  if constexpr (N == 32) { VIMA_WGMMA_K16(32, VIMA_R16, VIMA_ACC16, "%16", "%17", "%18"); }
+  else if constexpr (N == 64) { VIMA_WGMMA_K16(64, VIMA_R32, VIMA_ACC32, "%32", "%33", "%34"); }
+  else if constexpr (N == 96) { VIMA_WGMMA_K16(96, VIMA_R48, VIMA_ACC48, "%48", "%49", "%50"); }
+  else { VIMA_WGMMA_K16(128, VIMA_R64, VIMA_ACC64, "%64", "%65", "%66"); }
 }
-// e4m3 operands, both K-major in shared memory: M64 N64 K32
-__device__ __forceinline__ void wgmma_m64n64k32_e4m3_ss(float (&d)[32], uint64_t da, uint64_t db) {
-  asm volatile("wgmma.mma_async.sync.aligned.m64n64k32.f32.e4m3.e4m3 " VIMA_R32 ", %32, %33, 1, 1, 1;"
-               : VIMA_ACC32(d) : "l"(da), "l"(db));
+#undef VIMA_WGMMA_K16
+// e4m3 operands, both K-major in shared memory: M64 N{N} K32, always accumulating
+#define VIMA_WGMMA_E4M3(N, R, ACC, IA, IB)                                                                     \
+  asm volatile("wgmma.mma_async.sync.aligned.m64n" #N "k32.f32.e4m3.e4m3 " R ", " IA ", " IB ", 1, 1, 1;" \
+               : ACC(d) : "l"(da), "l"(db))
+template <int N>
+__device__ __forceinline__ void wgmma_m64nNk32_e4m3_ss(float (&d)[N / 2], uint64_t da, uint64_t db) {
+  static_assert(N == 32 || N == 64 || N == 96 || N == 128, "wgmma_m64nNk32_e4m3_ss: N is 32, 64, 96 or 128");
+  if constexpr (N == 32) { VIMA_WGMMA_E4M3(32, VIMA_R16, VIMA_ACC16, "%16", "%17"); }
+  else if constexpr (N == 64) { VIMA_WGMMA_E4M3(64, VIMA_R32, VIMA_ACC32, "%32", "%33"); }
+  else if constexpr (N == 96) { VIMA_WGMMA_E4M3(96, VIMA_R48, VIMA_ACC48, "%48", "%49"); }
+  else { VIMA_WGMMA_E4M3(128, VIMA_R64, VIMA_ACC64, "%64", "%65"); }
 }
+#undef VIMA_WGMMA_E4M3
+// warp-specialised register split: the producer warpgroup gives registers back, the consumer warpgroups take them
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 // A from registers (the 16-bit fragment of a previous accumulator), B K-major in shared memory: M64 N32 K16
 template <int DT>
 __device__ __forceinline__ void wgmma_m64n32k16_rs(float (&d)[16], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {

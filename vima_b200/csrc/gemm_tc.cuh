@@ -4,7 +4,11 @@
 //    pairs: in split mode the kernel accumulates A_hi*B_hi + A_lo*B_hi + A_hi*B_lo in the SAME fp32 register
 //    accumulator, which restores ~fp32 products (see DESIGN.md "operand precision").
 //  * Persistent, warp-specialised: warps 0-7 = two consumer warpgroups (rows [0,64) and [64,128) of the 128-row tile; each
-//    issues its wgmma M64 N64 instructions and runs the epilogue of its rows), warp 8 = TMA producer (one lane).
+//    issues one wgmma M64 N{BN} instruction per k step and operand pair and runs the epilogue of its rows), warps 8-11 = the
+//    producer warpgroup (one lane issues the TMA loads).  The producer warpgroup hands its registers to the consumers
+//    (setmaxnreg), which hold up to two 64 x 128 fp32 accumulators per warpgroup in f16f8 mode.
+//  * The split mode (SPLIT) and the tile width (BN) are template parameters, so every wgmma of the main loop is issued
+//    unconditionally: a wgmma under a run-time branch makes ptxas serialise the whole pipeline.
 //  * smem ring of `n_stages` stages {A_hi,[A_lo],B_hi,[B_lo]} in the 128-byte swizzled K-major layout that TMA
 //    writes and the wgmma descriptors read; the producer fills the next tile's stages while the consumers run the epilogue.
 //  * Epilogue: acc*scale + bias -> activation -> (GLU pair product) -> *mul -> +residual -> fp32 and/or (hi,lo).
@@ -19,9 +23,10 @@ constexpr int GEMM_BM = 128;
 constexpr int GEMM_BK = 64;                       // 64 x 2 B = 128 B = one swizzle row
 constexpr int GEMM_A_TILE_BYTES = GEMM_BM * 128;  // 16 KB
 constexpr int GEMM_CONSUMERS = 256;               // two warpgroups
-constexpr int GEMM_THREADS = GEMM_CONSUMERS + 32; // + the TMA producer warp
-constexpr int GEMM_MAX_BN = 128;                  // two 64-column accumulator chunks per thread (64 fp32 registers): with 9 warps
-                                                  // per CTA one SM sub-partition holds 3 of them, which caps a thread at 168 registers
+constexpr int GEMM_THREADS = GEMM_CONSUMERS + 128;  // + the producer warpgroup
+constexpr int GEMM_PRODUCER_REGS = 40;              // setmaxnreg split of the 64K-register file: 128 x 40 + 256 x 232 <= 65536
+constexpr int GEMM_CONSUMER_REGS = 232;
+constexpr int GEMM_MAX_BN = 128;                    // 64 fp32 accumulator registers per thread and accumulator
 constexpr int GEMM_MAX_STAGES = 8;
 constexpr int GEMM_STAGING_BYTES = 8 * 16 * 16 * 4;  // per-consumer-warp 16x16 fp32 transpose buffers (XOR-swizzled)
 
@@ -29,9 +34,7 @@ struct alignas(64) GemmParams {
   CUtensorMap tm_a_hi, tm_a_lo, tm_b_hi, tm_b_lo;  // in mode 2: tm_a_lo = A_lo8, tm_b_lo = B_lo8
   CUtensorMap tm_a_hi8, tm_b_hi8;                    // mode 2 only
   int M, N, K;      // N = accumulator columns (2x the output columns in GLU mode)
-  int block_n;      // multiple of 32 (64 in GLU mode), <= GEMM_MAX_BN
   int n_stages;
-  int split;        // 0: hi*hi only, 1: three-term fp16 split product, 2: fp16 hi*hi + two fp8 cross terms
   int dtype;        // DT_F16 / DT_BF16 (operand and 16-bit output format)
   int epi_prefetch; // 1: consumer warps pull the next tile's residual / multiplier rows into L2 one tile ahead
   int glu;          // 1: out[:, t*bn/2 + c] = act(acc[c]+bias[c]) * (acc[bn/2+c]+bias[bn/2+c]) per tile t
@@ -65,6 +68,8 @@ struct alignas(64) GemmParams {
 };
 
 // Compile-time epilogue description. GENERIC: every flag is read from GemmParams at run time instead.
+// The kernel's other template parameters: SPLIT (0: hi*hi only, 1: three-term fp16 split product, 2: fp16 hi*hi + two fp8 cross
+// terms) and BN (tile width: 32, 64, 96 or 128; 64 or 128 in GLU mode).
 template <bool GENERIC_, int ACT_, bool GLU_, bool MUL_, bool RES_, bool O32_, bool O16_, int DT_, bool LNA_ = false, bool LNR_ = false,
           bool STATS_ = false>
 struct EpiCfg {
@@ -91,14 +96,15 @@ __device__ __forceinline__ float act_ct(float x) {
 template <int DT>
 __device__ __forceinline__ void split4(const float4& y, uint2& hi, uint2& lo) { split4v<DT>(y, hi, lo); }
 
-// the 8 accumulator values of 16-column group s (columns 16s .. 16s+15) of this thread: the gate half of a GLU tile sits at a
-// run-time offset (block_n / 2), so its group index is only known at run time
-__device__ __forceinline__ void acc_group16(const float (&acc)[GEMM_MAX_BN / 64][32], int s, float (&v)[8]) {
+// the 8 accumulator values of 16-column group s (columns 16s .. 16s+15) of this thread: in the generic variant the gate half of
+// a GLU tile sits at a run-time offset (BN / 2 or not at all), so its group index is only known at run time
+template <int BN>
+__device__ __forceinline__ void acc_group16(const float (&acc)[BN / 2], int s, float (&v)[8]) {
 #pragma unroll
-  for (int t = 0; t < GEMM_MAX_BN / 16; ++t)
+  for (int t = 0; t < BN / 16; ++t)
     if (t == s) {
 #pragma unroll
-      for (int i = 0; i < 8; ++i) v[i] = acc[t >> 2][(t & 3) * 8 + i];
+      for (int i = 0; i < 8; ++i) v[i] = acc[t * 8 + i];
     }
 }
 
@@ -106,8 +112,9 @@ __device__ __forceinline__ void acc_group16(const float (&acc)[GEMM_MAX_BN / 64]
 // -> bias/act/GLU -> smem transpose (16x16 floats, 16-byte chunks XOR-swizzled by (row>>1)&3) -> [8 rows x 4 lanes x float4]
 // -> mul / residual / stores (128-bit fp32, 64-bit 16-bit pairs), issued after the sub-chunk's global loads are already in flight.
 // Row statistics keep the two column halves of the original layout: part 2*tn + ((column / 32) & 1).
-template <class E>
-__device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float (&acc)[GEMM_MAX_BN / 64][32], const float* __restrict__ sb,
+// acc is the m64nNk16 fragment: element 4*g + e holds column 8*g + 2*(lane % 4) + (e & 1), row 8*(e >> 1) + lane / 4.
+template <class E, int BN>
+__device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float (&acc)[BN / 2], const float* __restrict__ sb,
                                               float* __restrict__ st, int lane, int row_base, int tn, int bn_out, int n_out) {
   const bool glu = E::GENERIC ? (p.glu != 0) : E::GLU;
   const bool has_mul = E::GENERIC ? (p.mul != nullptr) : E::MUL;
@@ -167,7 +174,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float (
   load_mr(0, mm, rr);
   const int wsw = (sub >> 1) & 3;  // transpose swizzle of this thread's fragment rows (sub and sub + 8 share it)
 #pragma unroll
-  for (int s = 0; s < GEMM_MAX_BN / 16; ++s) {
+  for (int s = 0; s < BN / 16; ++s) {
     const int j = s * 16;
     if (j < bn_out) {
       const int col = tn * bn_out + j + kc * 4;
@@ -175,8 +182,8 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float (
       if (j + 16 < bn_out) load_mr(j + 16, mm_n, rr_n);
       float v[8], g[8], x[8];
 #pragma unroll
-      for (int i = 0; i < 8; ++i) v[i] = acc[s >> 2][(s & 3) * 8 + i];
-      if (glu) acc_group16(acc, s + bn_out / 16, g);
+      for (int i = 0; i < 8; ++i) v[i] = acc[s * 8 + i];
+      if (glu) acc_group16<BN>(acc, s + bn_out / 16, g);
       // fragment element i: row sub + 8*((i>>1)&1), column j + 8*(i>>2) + 2*kc + (i&1)
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
@@ -277,15 +284,15 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float (
   }
 }
 
-template <class E>
+template <class E, int SPLIT, int BN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_constant__ GemmParams p) {
+  static_assert(SPLIT >= 0 && SPLIT <= 2 && BN % 32 == 0 && BN <= GEMM_MAX_BN, "gemm_tc_kernel: bad SPLIT / BN");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // carve: [stages][staging][column vectors 2 x 4 x 256 f32][barriers]
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  const int BN = p.block_n;
-  const int b_tile_bytes = BN * 128;
-  const int n_parts = p.split ? 2 : 1;  // mode 2: the second "part" holds the two half-size fp8 tiles of each operand
-  const int stage_bytes = (GEMM_A_TILE_BYTES + b_tile_bytes) * n_parts;
+  constexpr int b_tile_bytes = BN * 128;
+  constexpr int n_parts = SPLIT ? 2 : 1;  // mode 2: the second "part" holds the two half-size fp8 tiles of each operand
+  constexpr int stage_bytes = (GEMM_A_TILE_BYTES + b_tile_bytes) * n_parts;
   uint8_t* stages = smem;
   float* staging = (float*)(smem + (size_t)p.n_stages * stage_bytes);
   float* sbias = staging + GEMM_STAGING_BYTES / 4;  // [2 buffers][GEMM_COLVEC_PLANES][256]
@@ -304,11 +311,11 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
   if (threadIdx.x == GEMM_CONSUMERS) {
     tma_prefetch_desc(&p.tm_a_hi);
     tma_prefetch_desc(&p.tm_b_hi);
-    if (p.split) {
+    if (SPLIT) {
       tma_prefetch_desc(&p.tm_a_lo);
       tma_prefetch_desc(&p.tm_b_lo);
     }
-    if (p.split == 2) {
+    if (SPLIT == 2) {
       tma_prefetch_desc(&p.tm_a_hi8);
       tma_prefetch_desc(&p.tm_b_hi8);
     }
@@ -320,9 +327,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
   }
   __syncthreads();
 
-  if (warp == GEMM_CONSUMERS / 32) {
+  if (warp >= GEMM_CONSUMERS / 32) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    setmaxnreg_dec<GEMM_PRODUCER_REGS>();
+    if (threadIdx.x == GEMM_CONSUMERS) {
       int stage = 0;
       uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -336,10 +344,10 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
           mbar_arrive_expect_tx(&full_bar[stage], (uint32_t)stage_bytes);
           tma_load_2d(st, &p.tm_a_hi, &full_bar[stage], k0, m0);
           tma_load_2d(sb, &p.tm_b_hi, &full_bar[stage], k0, n0);
-          if (p.split == 1) {
+          if (SPLIT == 1) {
             tma_load_2d(st + GEMM_A_TILE_BYTES, &p.tm_a_lo, &full_bar[stage], k0, m0);
             tma_load_2d(sb + b_tile_bytes, &p.tm_b_lo, &full_bar[stage], k0, n0);
-          } else if (p.split == 2) {  // [A_lo8 | A_hi8] and [B_hi8 | B_lo8]: 64-byte rows, half the fp16 tile each
+          } else if (SPLIT == 2) {  // [A_lo8 | A_hi8] and [B_hi8 | B_lo8]: 64-byte rows, half the fp16 tile each
             tma_load_2d(st + GEMM_A_TILE_BYTES, &p.tm_a_lo, &full_bar[stage], k0, m0);
             tma_load_2d(st + GEMM_A_TILE_BYTES + GEMM_A_TILE_BYTES / 2, &p.tm_a_hi8, &full_bar[stage], k0, m0);
             tma_load_2d(sb + b_tile_bytes, &p.tm_b_hi8, &full_bar[stage], k0, n0);
@@ -353,13 +361,13 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
   }
 
   // ===================== consumers: wgmma main loop + epilogue of rows [64*wg, +64) =====================
+  setmaxnreg_inc<GEMM_CONSUMER_REGS>();
   const int wg = warp >> 2;
   const int et = threadIdx.x;  // 0..255
   float* st = staging + warp * (16 * 16);
   const bool glu = E::GENERIC ? (p.glu != 0) : E::GLU;
   const int n_out = glu ? p.N / 2 : p.N;
   const int bn_out = glu ? BN / 2 : BN;
-  const int nch = (BN + 63) / 64;  // 64-column accumulator chunks in use (a chunk past BN reads rows beyond the B tile: discarded)
   const bool has_mul = E::GENERIC ? (p.mul != nullptr) : E::MUL;
   const bool has_res = E::GENERIC ? (p.residual != nullptr) : E::RES;
   // Pull a tile's multiplier / residual rows into L2 one tile ahead of its epilogue, so the epilogue's 128-bit
@@ -387,11 +395,13 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
     const int n0 = tn * BN;
     // the e4m3 cross terms get an accumulator of their own: fp8 wgmma adds its products into the accumulator with ~14 bits
     // kept, which would truncate these 2^-11-sized terms against the fp16 sum; their own sum is added in fp32 after the tile
-    float acc[GEMM_MAX_BN / 64][32], acc8[GEMM_MAX_BN / 64][32];
+    float acc[BN / 2], acc8[SPLIT == 2 ? BN / 2 : 1];
 #pragma unroll
-    for (int c = 0; c < GEMM_MAX_BN / 64; ++c)
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    if constexpr (SPLIT == 2) {
 #pragma unroll
-      for (int i = 0; i < 32; ++i) acc[c][i] = acc8[c][i] = 0.f;
+      for (int i = 0; i < BN / 2; ++i) acc8[i] = 0.f;
+    }
     int prev_stage = -1;
     for (int kb = 0; kb < num_kb; ++kb) {
       mbar_wait(&full_bar[stage], phase);
@@ -400,36 +410,29 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
       const uint64_t da_hi = wgmma_desc_sw128(a_hi + a_off);
       const uint64_t db_hi = wgmma_desc_sw128(b_hi);
       wgmma_fence();
+      // per accumulator element: every hi*hi step of the k block, then lo*hi and hi*lo per k step
 #pragma unroll
-      for (int k = 0; k < GEMM_BK / 16; ++k)  // +32 B per K=16 step inside the 128 B swizzle row; +8 KB per 64 B rows
-#pragma unroll
-        for (int c = 0; c < 4; ++c)
-          if (c < nch) wgmma_m64n64k16_ss<E::DT>(acc[c], da_hi + 2 * k, db_hi + 512 * c + 2 * k, 1u);
-      if (p.split == 1) {
+      for (int k = 0; k < GEMM_BK / 16; ++k)  // +32 B per K=16 step inside the 128 B swizzle row
+        wgmma_m64nNk16_ss<E::DT, BN>(acc, da_hi + 2 * k, db_hi + 2 * k, 1u);
+      if constexpr (SPLIT == 1) {
         const uint64_t da_lo = wgmma_desc_sw128(a_hi + GEMM_A_TILE_BYTES + a_off);
         const uint64_t db_lo = wgmma_desc_sw128(b_hi + b_tile_bytes);
 #pragma unroll
-        for (int k = 0; k < GEMM_BK / 16; ++k)
-#pragma unroll
-          for (int c = 0; c < GEMM_MAX_BN / 64; ++c)
-            if (c < nch) {
-              wgmma_m64n64k16_ss<E::DT>(acc[c], da_lo + 2 * k, db_hi + 512 * c + 2 * k, 1u);
-              wgmma_m64n64k16_ss<E::DT>(acc[c], da_hi + 2 * k, db_lo + 512 * c + 2 * k, 1u);
-            }
-      } else if (p.split == 2) {
+        for (int k = 0; k < GEMM_BK / 16; ++k) {
+          wgmma_m64nNk16_ss<E::DT, BN>(acc, da_lo + 2 * k, db_hi + 2 * k, 1u);
+          wgmma_m64nNk16_ss<E::DT, BN>(acc, da_hi + 2 * k, db_lo + 2 * k, 1u);
+        }
+      } else if constexpr (SPLIT == 2) {
         // cross terms at the fp8 rate: A_lo8 * B_hi8 and A_hi8 * B_lo8 (e4m3, K = 32 per instruction, 64-byte rows)
         const uint64_t da_lo8 = wgmma_desc_sw64(a_hi + GEMM_A_TILE_BYTES + a_off / 2);
         const uint64_t da_hi8 = wgmma_desc_sw64(a_hi + GEMM_A_TILE_BYTES + GEMM_A_TILE_BYTES / 2 + a_off / 2);
         const uint64_t db_hi8 = wgmma_desc_sw64(b_hi + b_tile_bytes);
         const uint64_t db_lo8 = wgmma_desc_sw64(b_hi + b_tile_bytes + b_tile_bytes / 2);
 #pragma unroll
-        for (int k = 0; k < GEMM_BK / 32; ++k)
-#pragma unroll
-          for (int c = 0; c < GEMM_MAX_BN / 64; ++c)
-            if (c < nch) {
-              wgmma_m64n64k32_e4m3_ss(acc8[c], da_lo8 + 2 * k, db_hi8 + 256 * c + 2 * k);
-              wgmma_m64n64k32_e4m3_ss(acc8[c], da_hi8 + 2 * k, db_lo8 + 256 * c + 2 * k);
-            }
+        for (int k = 0; k < GEMM_BK / 32; ++k) {
+          wgmma_m64nNk32_e4m3_ss<BN>(acc8, da_lo8 + 2 * k, db_hi8 + 2 * k);
+          wgmma_m64nNk32_e4m3_ss<BN>(acc8, da_hi8 + 2 * k, db_lo8 + 2 * k);
+        }
       }
       wgmma_commit();
       // keep this k block in flight; the previous one has retired -> its smem slot goes back to the producer
@@ -439,16 +442,11 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
       if (++stage == p.n_stages) { stage = 0; phase ^= 1; }
     }
     wgmma_wait<0>();
+    wgmma_fence_acc(acc);
+    if constexpr (SPLIT == 2) {
+      wgmma_fence_acc(acc8);
 #pragma unroll
-    for (int c = 0; c < GEMM_MAX_BN / 64; ++c) {
-      wgmma_fence_acc(acc[c]);
-      wgmma_fence_acc(acc8[c]);
-    }
-    if (p.split == 2) {
-#pragma unroll
-      for (int c = 0; c < GEMM_MAX_BN / 64; ++c)
-#pragma unroll
-        for (int i = 0; i < 32; ++i) acc[c][i] += acc8[c][i];
+      for (int i = 0; i < BN / 2; ++i) acc[i] += acc8[i];
     }
     if (prev_stage >= 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
     // per-column vectors of this tile -> smem (double-buffered: the other buffer may still be read by the slower warpgroup)
@@ -464,7 +462,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
       }
     }
     named_bar_sync(1, GEMM_CONSUMERS);
-    epilogue_tile<E>(p, acc, sb, st, lane, m0 + wg * 64 + (warp & 3) * 16, tn, bn_out, n_out);
+    epilogue_tile<E, BN>(p, acc, sb, st, lane, m0 + wg * 64 + (warp & 3) * 16, tn, bn_out, n_out);
     ab ^= 1;
   }
 }

@@ -1,6 +1,5 @@
+// gemm_tc_kernel instantiations of the "bf16" mode: bf16 operands, hi*hi only
 #include "gemm_tc_variants.cuh"
 namespace vima {
-cudaError_t launch_gemm_tc_bf16(const GemmParams& p, const GemmLaunch& l, int grid, size_t smem, int max_smem, cudaStream_t stream) {
-  return launch_gemm_tc_impl<DT_BF16>(p, l, grid, smem, max_smem, stream);
-}
+template cudaError_t launch_gemm_tc<DT_BF16, 0>(const GemmParams&, const GemmLaunch&, int, size_t, int, cudaStream_t);
 }  // namespace vima
