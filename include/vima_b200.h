@@ -25,7 +25,7 @@
  *     `vima_sizeof_*()` report the library's own sizes (bindings assert equality at load time).
  *   - the calling thread's current CUDA device is saved and restored around every call.
  *   - environment (read ONCE, in vima_create): VIMA_B200_ATTN = tc (default) | mma;  VIMA_B200_ATTN_TAIL = kernel (default) | off;
- *     VIMA_B200_EPI_PREFETCH = 0 (default) | 1.
+ *     VIMA_B200_EPI_PREFETCH = 0 (default) | 1;  VIMA_B200_ATTN_BIAS = auto (default) | tc.
  */
 #ifndef VIMA_B200_H
 #define VIMA_B200_H
@@ -56,7 +56,10 @@ int vima_sm_count(vima_ctx* ctx);
 /* Kernel-selection options, initialised from the environment in vima_create (see "environment" above) and switchable per context:
  * key "attn" = "tc" | "mma";  "attn_tail" = "kernel" | "off" (the <= 8 query rows past the last full 128-row tile: SIMT tail
  * kernel, or one more wgmma tile);
- * "epi_prefetch" = "1" | "0".  Unknown key/value: VIMA_E_INVALID. */
+ * "epi_prefetch" = "1" | "0";
+ * "attn_bias" = "auto" | "tc" (relative-bias attention, head_dim 64, non-causal -- the T5 encoder: "auto" runs the K/V-streaming
+ * wgmma kernel only where the resident-K/V kernel's shared memory does not fit, "tc" at every length; needs "attn" = "tc").
+ * Unknown key/value: VIMA_E_INVALID. */
 int vima_set_option(vima_ctx* ctx, const char* key, const char* value);
 /* sizeof() of the descriptor structs as THIS library was compiled (bindings check their mirror structs against these). */
 int vima_sizeof_gemm_desc(void);

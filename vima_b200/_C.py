@@ -176,7 +176,9 @@ class Context:
             raise RuntimeError(f"{what} failed (code {rc}): {msg.decode() if msg else ''}")
 
     def set_option(self, key: str, value: str) -> None:
-        """Kernel selection of this context: attn = tc | mma, attn_tail = kernel | off, epi_prefetch = 1 | 0."""
+        """Kernel selection of this context: attn = tc | mma, attn_tail = kernel | off, epi_prefetch = 1 | 0, attn_bias = auto | tc
+        (relative-bias attention, i.e. the T5 encoder, on the K/V-streaming wgmma kernel only past the resident-K/V kernel's
+        shared memory, or at every length)."""
         self._ck(self.lib.vima_set_option(self.h, key.encode(), str(value).encode()), "set_option")
 
     @property

@@ -25,6 +25,8 @@ struct vima_ctx {
   int attn_tail;     // VIMA_B200_ATTN_TAIL: the <= 8 rows past the last full 128-row tile: 1 = "kernel" (default; SIMT tail kernel),
                      // 0 = "off" (one more tensor-core tile)
   int epi_prefetch;  // VIMA_B200_EPI_PREFETCH: L2 prefetch of the next tile's residual / multiplier rows (default 0)
+  int attn_bias_tc;  // VIMA_B200_ATTN_BIAS: relative-bias attention (T5) on the streaming wgmma kernel: 0 = "auto" (default; only past the
+                     // resident-K/V kernel's shared memory), 1 = "tc" (at every length)
 };
 
 // Restores the calling thread's CUDA device when an entry point returns (the library switches to the context's device).
@@ -101,6 +103,9 @@ int vima_set_option(vima_ctx* c, const char* key, const char* value) {
   } else if (!strcmp(key, "attn_tail")) {
     if (!strcmp(value, "kernel")) { c->attn_tail = 1; return VIMA_OK; }
     if (!strcmp(value, "off")) { c->attn_tail = 0; return VIMA_OK; }
+  } else if (!strcmp(key, "attn_bias")) {
+    if (!strcmp(value, "auto")) { c->attn_bias_tc = 0; return VIMA_OK; }
+    if (!strcmp(value, "tc")) { c->attn_bias_tc = 1; return VIMA_OK; }
   } else if (!strcmp(key, "epi_prefetch")) {
     if (!strcmp(value, "0") || !strcmp(value, "1")) { c->epi_prefetch = value[0] == '1'; return VIMA_OK; }
   }
@@ -130,10 +135,11 @@ int vima_create(vima_ctx** out, int device) {
     return VIMA_E_CUDA;
   }
   c->encode_tiled = fn;
-  c->attn_tc = 1; c->attn_tail = 1; c->epi_prefetch = 0;
+  c->attn_tc = 1; c->attn_tail = 1; c->epi_prefetch = 0; c->attn_bias_tc = 0;
   if (const char* e = getenv("VIMA_B200_ATTN")) vima_set_option(c, "attn", e);  // unknown values keep the default
   if (const char* e = getenv("VIMA_B200_ATTN_TAIL")) vima_set_option(c, "attn_tail", e);
   if (const char* e = getenv("VIMA_B200_EPI_PREFETCH")) vima_set_option(c, "epi_prefetch", e);
+  if (const char* e = getenv("VIMA_B200_ATTN_BIAS")) vima_set_option(c, "attn_bias", e);
   c->err[0] = 0;
   *out = c;
   return VIMA_OK;
@@ -411,6 +417,10 @@ int vima_attention(vima_ctx* c, const vima_attn_desc* d_in, void* stream) {
     }
     LAUNCHED(c, launch_attention_tc(p, c->encode_tiled, (cudaStream_t)stream), "attention_tc");
   }
+  // T5's relative-bias attention (head_dim 64, non-causal): the streaming wgmma kernel takes every length the resident-K/V kernel
+  // cannot hold, and every length with attn_bias=tc.  Everything that fits stays on the mma.sync kernel below by default.
+  if (c->attn_tc && attention_bias_tc_supported(p) && (c->attn_bias_tc || attention_smem_bytes(p) > (size_t)c->max_smem_optin))
+    LAUNCHED(c, launch_attention_bias_tc(p, c->encode_tiled, (cudaStream_t)stream), "attention_bias_tc");
   {
     // the mma.sync kernel keeps K and V^T (hi + lo) of one (batch, head) resident in shared memory
     const size_t need = attention_smem_bytes(p);

@@ -42,28 +42,6 @@ struct AttnTcParams {
   CUtensorMap tm_q_hi, tm_q_lo, tm_k_hi, tm_k_lo;
 };
 
-__device__ __forceinline__ unsigned short e4m3x2(float x0, float x1) {  // low byte = x0
-  unsigned short r;
-  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(x1), "f"(x0));
-  return r;
-}
-
-// two adjacent output values of one query row: (hi, lo) 16-bit pairs [+ e4m3 cross-term views for an "f16f8" consumer GEMM]
-template <int DT>
-__device__ __forceinline__ void store_pair(const AttnParams& p, size_t brow, int col, float x0, float x1) {
-  uint32_t hi, lo;
-  split2<DT>(x0, x1, hi, lo);
-  const size_t off = brow * p.ldo + col;
-  *reinterpret_cast<uint32_t*>(p.o_hi + off) = hi;
-  if (p.o_lo) *reinterpret_cast<uint32_t*>(p.o_lo + off) = lo;
-  if (p.o_lo8) {
-    const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hi));
-    const size_t off8 = brow * p.ldo8 + col;
-    *reinterpret_cast<unsigned short*>(p.o_lo8 + off8) = e4m3x2((x0 - f.x) * F8_ACT_LO_SCALE, (x1 - f.y) * F8_ACT_LO_SCALE);
-    *reinterpret_cast<unsigned short*>(p.o_hi8 + off8) = e4m3x2(x0 * F8_ACT_HI_SCALE, x1 * F8_ACT_HI_SCALE);
-  }
-}
-
 template <int DT>
 __global__ void __launch_bounds__(ATC_THREADS, 2) attention_tc_kernel(const __grid_constant__ AttnTcParams P) {
   const AttnParams& p = P.a;
@@ -255,7 +233,7 @@ __global__ void __launch_bounds__(ATC_THREADS, 2) attention_tc_kernel(const __gr
       const float inv = 1.0f / l;
       const size_t brow = (size_t)b * qbr + row;
 #pragma unroll
-      for (int g = 0; g < 4; ++g) store_pair<DT>(p, brow, x_col + 8 * g + 2 * qd, o[4 * g + 2 * hh] * inv, o[4 * g + 2 * hh + 1] * inv);
+      for (int g = 0; g < 4; ++g) attn_store_pair<DT>(p, brow, x_col + 8 * g + 2 * qd, o[4 * g + 2 * hh] * inv, o[4 * g + 2 * hh + 1] * inv);
     }
   }
 }

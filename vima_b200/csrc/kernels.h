@@ -48,12 +48,34 @@ __device__ __forceinline__ void attn_batch_keys(const AttnParams& p, int b, int 
     lk = max(min(qp0 + qbr, p.Lk), 1);
   }
 }
-constexpr int ATTN_TAIL_MAX_ROWS = 8;          // attention_tail.cu: query rows per (batch, head) the SIMT tail kernel takes
+// two adjacent output values of one query row (the wgmma attention kernels): (hi, lo) 16-bit pairs [+ e4m3 cross-term views for an
+// "f16f8" consumer GEMM]
+template <int DT>
+__device__ __forceinline__ void attn_store_pair(const AttnParams& p, size_t brow, int col, float x0, float x1) {
+  uint32_t hi, lo;
+  split2<DT>(x0, x1, hi, lo);
+  const size_t off = brow * p.ldo + col;
+  *reinterpret_cast<uint32_t*>(p.o_hi + off) = hi;
+  if (p.o_lo) *reinterpret_cast<uint32_t*>(p.o_lo + off) = lo;
+  if (p.o_lo8) {
+    const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&hi));
+    const size_t off8 = brow * p.ldo8 + col;
+    unsigned short l8, h8;  // low byte = x0
+    asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(l8) : "f"((x1 - f.y) * F8_ACT_LO_SCALE), "f"((x0 - f.x) * F8_ACT_LO_SCALE));
+    asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(h8) : "f"(x1 * F8_ACT_HI_SCALE), "f"(x0 * F8_ACT_HI_SCALE));
+    *reinterpret_cast<unsigned short*>(p.o_lo8 + off8) = l8;
+    *reinterpret_cast<unsigned short*>(p.o_hi8 + off8) = h8;
+  }
+}
+constexpr int ATTN_TAIL_MAX_ROWS = 8;         // attention_tail.cu: query rows per (batch, head) the SIMT tail kernel takes
 cudaError_t launch_attention(const AttnParams& p, cudaStream_t stream);
 size_t attention_smem_bytes(const AttnParams& p);             // dynamic shared memory the mma.sync kernel needs for p
 int attention_max_lk(const AttnParams& p, size_t smem_limit);  // largest Lk (multiple of 64) that fits smem_limit at p's format
 bool attention_tc_supported(const AttnParams& p);  // wgmma variant (attention_tc.cu): head_dim 32, split operands, no bias, Lk <= 512
 cudaError_t launch_attention_tc(const AttnParams& p, void* encode_tiled_fn, cudaStream_t stream);  // encode_tiled_fn: cuTensorMapEncodeTiled
+// wgmma variant for the T5 encoder (attention_bias_tc.cu): head_dim 64, relative bias, non-causal, K/V streamed (no length cap)
+bool attention_bias_tc_supported(const AttnParams& p);
+cudaError_t launch_attention_bias_tc(const AttnParams& p, void* encode_tiled_fn, cudaStream_t stream);
 // query rows [row0, row0 + nt) of every (batch, head) (nt <= ATTN_TAIL_MAX_ROWS, head_dim 32, Lk <= 512): the rows that would
 // otherwise occupy a nearly empty 128-row tile of the wgmma kernel
 cudaError_t launch_attention_tail(const AttnParams& p, int row0, int nt, cudaStream_t stream);
