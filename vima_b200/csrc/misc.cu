@@ -479,6 +479,9 @@ __global__ void head_select_kernel(const float* __restrict__ logits, int B, int 
     const int oi = __shfl_xor_sync(0xffffffffu, best_i, o);
     if (ob > best || (ob == best && oi < best_i)) { best = ob; best_i = oi; }
   }
+  // a head whose logits are all -inf has NaN probabilities (and NaN normalised logits, as log_softmax gives): argmax over
+  // them is index 0 in torch, and no lane found a probability to keep
+  if (best_i == 0x7fffffff) best_i = 0;
   if (lane == 0) modes[(size_t)b * n_heads + hd] = (long long)best_i;
 }
 cudaError_t launch_head_select(const float* logits, int B, int n_heads, const int* head_off, float* logits_norm, long long* modes,
