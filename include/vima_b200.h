@@ -151,7 +151,10 @@ int vima_row_stats_finalize(vima_ctx*, const float* partial, int64_t rows, int p
 
 /* ---- exact fp32 grouped GEMM (CUDA cores) for the tiny layers -------------------------------------------------
  * action_decoder.py:151-166 (12 MLPs E->512->512->{50|100}), action_embd.py:29-56, obj_encoder.py:86 first layer.
- * `groups` is a DEVICE array of n_groups descriptors; y[M, n] = act(x[M, k] * w[n, k]^T + b). */
+ * `groups` is a DEVICE array of n_groups descriptors; y[M, n] = act(x[M, k] * w[n, k]^T + b).  Every output accumulates its
+ * products in ascending k with one fused multiply-add each, then adds b in fp32: bit for bit the same at any M or grouping.
+ * Precondition: max_n >= every group's n.  max_n sets the launch's column tiles, so the columns of a wider group past max_n are
+ * never written; the descriptors live on the device, so this entry point cannot check it. */
 typedef struct {
   const float* x; int ldx;
   const float* w; int ldw;
@@ -161,7 +164,8 @@ typedef struct {
 } vima_f32_gemm_group;
 int vima_gemm_f32_grouped(vima_ctx*, const vima_f32_gemm_group* groups_dev, int n_groups, int M, int max_n, int act, void* stream);
 /* Same, with the descriptor array in HOST memory: the descriptors travel in the kernel's parameter space (16 per launch), so no
- * device-side array has to stay alive and the call can be captured into a CUDA graph. */
+ * device-side array has to stay alive and the call can be captured into a CUDA graph.  Returns VIMA_E_INVALID, and launches
+ * nothing, when M < 0 or a group's n exceeds max_n. */
 int vima_gemm_f32_grouped_host(vima_ctx*, const vima_f32_gemm_group* groups_host, int n_groups, int M, int max_n, int act, void* stream);
 
 /* ---- LayerNorm / T5 RMSNorm over rows ---------------------------------------------------------------------

@@ -339,6 +339,11 @@ int vima_gemm_f32_grouped(vima_ctx* c, const vima_f32_gemm_group* groups_dev, in
 int vima_gemm_f32_grouped_host(vima_ctx* c, const vima_f32_gemm_group* groups_host, int n_groups, int M, int max_n, int act, void* stream) {
   CHECK_CTX(c);
   if (!groups_host || n_groups < 0) return fail(c, VIMA_E_INVALID, "gemm_f32_grouped_host: null groups");
+  if (M < 0) return fail(c, VIMA_E_INVALID, "gemm_f32_grouped_host: M = %d < 0", M);
+  // max_n sizes the grid's column tiles: a group with more columns would have its last ones silently never written
+  for (int i = 0; i < n_groups; ++i)
+    if (groups_host[i].n > max_n)
+      return fail(c, VIMA_E_INVALID, "gemm_f32_grouped_host: group %d has n = %d columns, more than max_n = %d", i, groups_host[i].n, max_n);
   cudaError_t e = launch_simt_gemm_grouped_host(reinterpret_cast<const SimtGemmGroup*>(groups_host), n_groups, M, max_n, act, (cudaStream_t)stream);
   if (e != cudaSuccess) return cuda_fail(c, e, "simt_gemm");
   c->launches += (n_groups + SIMT_MAX_HOST_GROUPS - 1) / SIMT_MAX_HOST_GROUPS;
