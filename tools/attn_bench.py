@@ -1,15 +1,25 @@
-"""GPU microbenchmark of attention_kernel at the cfg3 decoder shapes (B=256, H=24, d=32, L=263, Lp=256)."""
+"""GPU microbenchmark of decoder attention at the cfg3 shapes (B=256, H=24, d=32, L=263, Lp=256).
+
+Environment: AB_B episodes, AB_L history keys (causal self-attention, Lq = Lk = L), AB_LP cross-attention keys (prompt tokens, Lq = L),
+AB_LQ > 0 adds a decode case (AB_LQ new query rows over AB_L cached keys, queries last), AB_SPLIT formats, AB_MASKED.
+"""
 import sys, os, math
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from vima_b200 import _C
 ctx = _C.Context.get(torch.device("cuda", 0))
-B, H, D, L, Lp = int(os.environ.get("AB_B", 256)), 24, 32, int(os.environ.get("AB_L", 263)), 256
+B, H, D, L, Lp = int(os.environ.get("AB_B", 256)), 24, 32, int(os.environ.get("AB_L", 263)), int(os.environ.get("AB_LP", 256))
+Ld = int(os.environ.get("AB_LQ", 0))
 E = H * D
+cases = [("self causal", L, L, True), ("cross", L, Lp, False)] + ([(f"decode Lq={Ld}", Ld, L, True)] if Ld > 0 else [])
 for split in [int(x) for x in os.environ.get("AB_SPLIT", "0,1").split(",")]:
-    for name, Lq, Lk, causal in (("self causal", L, L, True), ("cross", L, Lp, False)):
+    for name, Lq, Lk, causal in cases:
         mk = lambda r, c: torch.randint(-3000, 3000, (r, c), dtype=torch.int16, device="cuda")
-        if causal:
+        if causal and Lq < Lk:  # decode: the new rows' queries over the cached keys
+            qq = mk(B * Lq, E); ql = mk(B * Lq, E) if split else None
+            kv = mk(B * Lk, 2 * E); kl = mk(B * Lk, 2 * E) if split else None
+            q = (qq, ql, E, 0); k = (kv, kl, 2 * E, 0); v = (kv, kl, 2 * E, E)
+        elif causal:
             qkv = mk(B * Lq, 3 * E); qkl = mk(B * Lq, 3 * E) if split else None
             q = (qkv, qkl, 3 * E, 0); k = (qkv, qkl, 3 * E, E); v = (qkv, qkl, 3 * E, 2 * E)
         else:
@@ -21,12 +31,16 @@ for split in [int(x) for x in os.environ.get("AB_SPLIT", "0,1").split(",")]:
         if causal and os.environ.get("AB_MASKED", "1") == "1":  # the bench workload pads ~10 % of the history's object slots
             mask = (torch.rand(B, Lk, device="cuda") > 0.1).to(torch.uint8)
             mask[:, 0] = 1
-        kw = dict(q=q, k=k, v=v, o=(o_hi, o_lo, E, 0), B=B, H=H, Lq=Lq, Lk=Lk, D=D, scale=1 / math.sqrt(D), causal=causal, key_mask=mask, dtype=0)
+        kw = dict(q=q, k=k, v=v, o=(o_hi, o_lo, E, 0), B=B, H=H, Lq=Lq, Lk=Lk, D=D, scale=1 / math.sqrt(D), causal=causal, key_mask=mask, dtype=0,
+                  q_pos0=Lk - Lq if causal else 0)
         ctx.attention(**kw); torch.cuda.synchronize()
         e0 = torch.cuda.Event(enable_timing=True); e1 = torch.cuda.Event(enable_timing=True)
         e0.record()
         for _ in range(5): ctx.attention(**kw)
         e1.record(); torch.cuda.synchronize()
         ms = e0.elapsed_time(e1) / 5
-        fl = 4.0 * B * H * Lq * Lk * D * (0.5 if causal else 1.0)
-        print(f"split={split} {name:12s} {ms:7.3f} ms   {fl/ms/1e9:7.1f} TF/s algorithmic (causal counted as half)", flush=True)
+        # causal: the cached keys in full plus half the square of the new rows (half of Lq * Lk for Lq = Lk)
+        pairs = Lq * (Lk - Lq) + Lq * Lq / 2 if causal else Lq * Lk
+        fl = 4.0 * B * H * pairs * D
+        print(f"split={split} {name:12s} Lq={Lq:5d} Lk={Lk:5d} {ms:8.3f} ms   {fl/ms/1e9:7.1f} TF/s algorithmic (causal: visible half of the new rows' square)",
+              flush=True)

@@ -13,6 +13,9 @@ positions).  Every episode runs to its end in each of three runs, and each run r
   eager     open_slots / step_slots: a slot whose episode ended takes the next episode before the next tick (admit), or is released
   graph     the same schedule with the step replayed from one CUDA graph (capture time reported, not counted)
 
+Longer episodes need more decoder positions: `--policy gato --model gato_200M --n-positions 1024 --max-steps 45` gives each slot
+257 + 45 * 17 = 1022 columns.  The header line prints the K/V cache size (n_layer * S * Lmax * 2E * 4 bytes).
+
 Admission (the prompt key/value GEMMs of the new episodes) is included in the slot runs' totals and also reported on its own
 (CUDA events).  Weights are random (timing only).  Prints the GPU's name and power limit beside the numbers, one JSON line per run.
 """
@@ -48,6 +51,8 @@ def main():
     ap.add_argument("--n-obj", type=int, default=32)
     ap.add_argument("--prompt-len", type=int, default=256)
     ap.add_argument("--max-steps", type=int, default=15)
+    ap.add_argument("--n-positions", type=int, default=None,
+                    help="decoder positions (default: the policy's 512); gato / gpt: the constructor's n_positions, vima: XAttnGPT rebuilt")
     ap.add_argument("--episodes", type=int, default=1024)
     ap.add_argument("--precision", default="f16f8")
     ap.add_argument("--seed", type=int, default=0)
@@ -58,13 +63,24 @@ def main():
     vima_b200.set_precision(a.precision)
     torch.manual_seed(a.seed)
     vima = a.policy == "vima"
+    npos = {} if a.n_positions is None else {"n_positions": a.n_positions}
     if vima:
-        pol = vima_b200.VIMAPolicy(**synth.MODEL_CFGS[a.model or "200M"]).cuda().eval()
+        cfg = synth.MODEL_CFGS[a.model or "200M"]
+        pol = vima_b200.VIMAPolicy(**cfg)
+        if npos:
+            from vima_b200 import nn as vnn
+
+            pol.xattn_gpt = vnn.XAttnGPT(cfg["embed_dim"], n_layer=cfg["xf_n_layers"], n_head=cfg["sattn_n_heads"], dropout=0.1,
+                                         xattn_n_head=cfg["xattn_n_heads"], xattn_ff_expanding=4, xattn_n_positions=256, use_geglu=True,
+                                         **npos)
+        pol = pol.cuda().eval()
     elif a.policy == "flamingo":
+        if npos:
+            raise SystemExit("--n-positions applies to --policy vima, gato and gpt")
         pol = vima_b200.VIMAFlamingoPolicy(**synth.FLAMINGO_CFGS[a.model or "flamingo_tiny"]).cuda().eval()
     else:
         cls = vima_b200.VIMAGatoPolicy if a.policy == "gato" else vima_b200.VIMAGPTPolicy
-        pol = cls(**synth.GATO_CFGS[a.model or "gato_200M"]).cuda().eval()
+        pol = cls(**synth.GATO_CFGS[a.model or "gato_200M"], **npos).cuda().eval()
     E, S, Lp = pol.embed_dim, a.slots, a.prompt_len
     Q = a.n_obj if vima else pol._obj_xf_num_queries
     prefix = Lp + 1 if a.policy in ("gato", "gpt") else 0  # the decoder-only caches hold prompt + separator
@@ -82,8 +98,10 @@ def main():
     pmask = torch.ones(S, Lp, dtype=torch.bool, device="cuda")
     info = gpu_info()
     name = "" if vima else f"policy {a.policy}, "
+    n_layer = pol.xattn_gpt.n_layer if hasattr(pol, "xattn_gpt") else pol.transformer.n_layer
+    kv_bytes = n_layer * S * Lmax * 2 * E * 4  # per layer [S*Lmax, 2E] K|V as (hi, lo) 16-bit pairs
     print(f"# {info}; {name}model {a.model or '200M'}, {S} slots, Q={Q}, Lp={Lp}, {a.precision}; {a.episodes} episodes of 1..{a.max_steps} steps "
-          f"({total_steps} env-steps, seed {a.seed})")
+          f"({total_steps} env-steps, seed {a.seed}); {Lmax} cache columns per slot, K/V cache {kv_bytes / 1e9:.2f} GB")
 
     if vima:
         forward_step, step_slots = pol.forward_step, pol.step_slots
@@ -202,6 +220,8 @@ def main():
                 r["admission_ms_per_episode"] = round(adm / len(lengths), 4)
             r.update(extra)
             r["gpu"] = info
+            r["cache_columns"] = Lmax
+            r["kv_cache_bytes"] = kv_bytes
             results.append(r)
             print(json.dumps(r), flush=True)
 

@@ -409,9 +409,10 @@ int vima_attention(vima_ctx* c, const vima_attn_desc* d_in, void* stream) {
   // VIMA_B200_ATTN=mma (read once in vima_create) forces the latter.  Both are covered by the kernel tests.
   if (c->attn_tc && attention_tc_supported(p)) {
     // the wgmma kernel works on 128-row query tiles: a few rows past the last full tile (7 of 263, 8 of 392) would hold a CTA slot
-    // for the whole key range with one warp of eight at work -- they go to the SIMT tail kernel instead (attention_tail.cu).
+    // for the whole key range with one warp of eight at work -- they go to the SIMT tail kernel instead (attention_tail.cu), as
+    // long as its shared memory holds the key range; past that they run in the wgmma kernel's last tile.
     const int tail = p.Lq % 128;
-    if (c->attn_tail && p.Lq > 128 && tail >= 1 && tail <= ATTN_TAIL_MAX_ROWS) {
+    if (c->attn_tail && p.Lq > 128 && tail >= 1 && tail <= ATTN_TAIL_MAX_ROWS && p.Lk <= ATTN_TAIL_MAX_LK) {
       AttnParams body = p;
       body.Lq = p.Lq - tail;
       body.q_batch_rows = p.Lq;

@@ -1,4 +1,6 @@
-// Fused masked attention for the VIMA decoder / T5 encoder (head_dim 32 or 64, sequences <= 512).
+// Fused masked attention, K and V^T resident in shared memory (head_dim 32 or 64; Lk up to what the device's shared memory holds,
+// attention_max_lk).  It runs what the streaming wgmma kernels do not take: single-pass f16 / bf16 operands, the decoder at
+// head_dim 64, and the T5 encoder's prompts that fit.
 //
 //   S = scale * Q K^T (+ T5 relative bias) ; causal: S[i][j>i] = -1e4 (the reference's soft mask,
 //   components.py:61-63) ; S += (key_mask ? 0 : finfo(fp32).min) ; P = softmax(S) ; O = P V

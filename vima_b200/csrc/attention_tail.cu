@@ -241,7 +241,7 @@ cudaError_t launch_attention_tail(const AttnParams& p, int row0, int nt, cudaStr
   if (nt > TAIL_NT || p.D != TAIL_D) return cudaErrorInvalidValue;
   const int lk_pad = (p.Lk + 31) & ~31;
   const size_t smem = (size_t)TAIL_WARPS * (TAIL_NT * TAIL_D + (size_t)lk_pad * TAIL_NT) * sizeof(float);
-  constexpr size_t smem_max = (size_t)TAIL_WARPS * (TAIL_NT * TAIL_D + 512 * TAIL_NT) * sizeof(float);  // Lk <= 512 (attention_tc's limit)
+  constexpr size_t smem_max = (size_t)TAIL_WARPS * (TAIL_NT * TAIL_D + (size_t)ATTN_TAIL_MAX_LK * TAIL_NT) * sizeof(float);
   if (smem > smem_max) return cudaErrorInvalidValue;
   static bool attr_set[2][64] = {};  // once per (format, device): not legal inside a CUDA-graph capture
   int dev = 0;

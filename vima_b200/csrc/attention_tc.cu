@@ -5,7 +5,8 @@
 //     S[64x64] = Q K^T     6 x wgmma M64 N64 K16 (hi*hi, lo*hi, hi*lo), Q and K(c) from shared memory (TMA, 64-byte swizzle);
 //                          K(c+2) is loaded by TMA into the slot K(c) leaves
 //     V(c) -> V^T          while S is computed, every thread loads 8 values of V(c) (hi and lo) and writes them transposed into
-//                          a 128-byte-swizzled K-major tile, the B operand layout wgmma reads
+//                          a 128-byte-swizzled K-major tile, the B operand layout wgmma reads; it also stages chunk c+1's 64
+//                          key-mask terms in a double buffer, so no shared memory is sized by Lk (no length cap)
 //     softmax              in registers on the accumulator fragment (4 lanes share a row), online maximum, exp2 with the scale
 //                          folded into the FMA; P as (hi, lo) 16-bit pairs stays in registers
 //     O[64x32] += P V      12 x wgmma M64 N32 K16 with A = P from registers, B = V^T from shared memory
@@ -28,13 +29,12 @@ constexpr float EXIT_L2_TC = -9000.f * LOG2E_TC;
 
 constexpr int ATC_THREADS = 256;
 constexpr int ATC_BM = 128, ATC_KC = 64, ATC_D = 32;
-constexpr int ATC_MAX_LK = 512;      // mask row held in shared memory as floats
 // shared memory carve (bytes; swizzled tiles 1024-aligned)
 constexpr int OFF_QH = 0, OFF_QL = 8192;     // 128 rows x 64 B each
 constexpr int OFF_K = 16384;                 // 2 stages x {hi 4096, lo 4096}: 64 keys x 64 B
 constexpr int OFF_VT = 32768;                // 2 buffers x {hi 4096, lo 4096}: V^T, 32 dims x 128 B
-constexpr int OFF_MASK = 49152;              // float[512]
-constexpr int OFF_BAR = OFF_MASK + ATC_MAX_LK * 4;  // 3 mbarriers
+constexpr int OFF_MASK = 49152;              // float[2][64]: key-mask terms of a chunk
+constexpr int OFF_BAR = OFF_MASK + 2 * ATC_KC * 4;  // 3 mbarriers
 constexpr int ATC_SMEM = OFF_BAR + 32;
 
 struct AttnTcParams {
@@ -46,7 +46,7 @@ template <int DT>
 __global__ void __launch_bounds__(ATC_THREADS, 2) attention_tc_kernel(const __grid_constant__ AttnTcParams P) {
   const AttnParams& p = P.a;
   extern __shared__ __align__(1024) uint8_t sm[];
-  float* maskadd = reinterpret_cast<float*>(sm + OFF_MASK);
+  float* maskadd = reinterpret_cast<float*>(sm + OFF_MASK);  // [2][64]
   uint64_t* bars = reinterpret_cast<uint64_t*>(sm + OFF_BAR);
   uint64_t* q_full = bars + 0;
   uint64_t* k_full = bars + 1;  // [2]
@@ -84,12 +84,16 @@ __global__ void __launch_bounds__(ATC_THREADS, 2) attention_tc_kernel(const __gr
     tma_prefetch_desc(&P.tm_q_hi); tma_prefetch_desc(&P.tm_q_lo);
     tma_prefetch_desc(&P.tm_k_hi); tma_prefetch_desc(&P.tm_k_lo);
   }
-  // key mask row of this batch element as additive terms
-  for (int j = tid; j < n_all * ATC_KC; j += ATC_THREADS) {
-    float mk = -INFINITY;  // beyond the sequence: excluded
-    if (j < Lk) mk = (p.key_mask == nullptr || p.key_mask[(size_t)b * mld + j]) ? 0.f : FP32_MIN_TC;
-    maskadd[j] = mk;
-  }
+  // chunk c's key-mask terms of this batch element into buffer c & 1 (threads 192..255, one key each)
+  auto stage_mask = [&](int c) {
+    if (tid >= ATC_THREADS - ATC_KC) {
+      const int j = c * ATC_KC + tid - (ATC_THREADS - ATC_KC);
+      float mk = -INFINITY;  // beyond the sequence: excluded
+      if (j < Lk) mk = (p.key_mask == nullptr || p.key_mask[(size_t)b * mld + j]) ? 0.f : FP32_MIN_TC;
+      maskadd[(c & 1) * ATC_KC + tid - (ATC_THREADS - ATC_KC)] = mk;
+    }
+  };
+  stage_mask(0);
   __syncthreads();
 
   auto load_k = [&](int c, int stage) {  // thread 0 only
@@ -149,6 +153,7 @@ __global__ void __launch_bounds__(ATC_THREADS, 2) attention_tc_kernel(const __gr
           vh = __ldg(reinterpret_cast<const uint4*>(p.v_hi + off));
           vl = __ldg(reinterpret_cast<const uint4*>(p.v_lo + off));
         }
+        if (c + 1 < n) stage_mask(c + 1);  // read after the barrier below; buffer (c+1)&1 was last read before the previous one
         uint8_t* vt = sm + OFF_VT + stage * 8192;
         const uint32_t wh[4] = {vh.x, vh.y, vh.z, vh.w}, wl[4] = {vl.x, vl.y, vl.z, vl.w};
 #pragma unroll
@@ -163,13 +168,14 @@ __global__ void __launch_bounds__(ATC_THREADS, 2) attention_tc_kernel(const __gr
       wgmma_wait<0>();
       wgmma_fence_acc(s);
       // ---- softmax on the fragment: element 4g+e is row r_loc + 8*(e>>1), key k0 + 8g + 2qd + (e&1) ----
+      const float* mk = maskadd + stage * ATC_KC;
       float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
       for (int g = 0; g < 8; ++g)
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-          const int key = k0 + 8 * g + 2 * qd + (e & 1);
-          const float mm = maskadd[key];
+          const int jj = 8 * g + 2 * qd + (e & 1), key = k0 + jj;
+          const float mm = mk[jj];
           float y = fmaf(s[4 * g + e], c_l2, mm);
           if (p.causal && key > q0 + r_loc + 8 * (e >> 1) + qp0) y = CAUSAL_L2_TC + mm;
           s[4 * g + e] = y;
@@ -197,7 +203,7 @@ __global__ void __launch_bounds__(ATC_THREADS, 2) attention_tc_kernel(const __gr
       for (int hh = 0; hh < 2; ++hh) l_run[hh] = l_run[hh] * f[hh] + ps[hh];
 #pragma unroll
       for (int i = 0; i < 16; ++i) o[i] *= f[(i >> 1) & 1];
-      // V^T(c) is complete, and both warpgroups are done reading K(c): its slot takes K(c+2)
+      // V^T(c) and chunk c+1's mask terms are complete, and both warpgroups are done reading K(c): its slot takes K(c+2)
       named_bar_sync(1, ATC_THREADS);
       if (tid == 0 && c + 2 < n) load_k(c + 2, stage);
       {
@@ -221,6 +227,8 @@ __global__ void __launch_bounds__(ATC_THREADS, 2) attention_tc_kernel(const __gr
     const int undone = (r_loc < rows_here && !(m_run[0] > EXIT_L2_TC)) || (r_loc + 8 < rows_here && !(m_run[1] > EXIT_L2_TC));
     if (!__syncthreads_or(undone)) break;
     n = n_all;
+    stage_mask(0);  // every read of pass 0's mask buffers precedes the barrier above
+    __syncthreads();
   }
   // ---- normalise and store (hi, lo) [+ e4m3 views] ----
 #pragma unroll
@@ -258,12 +266,14 @@ static bool make_map(void* encode, CUtensorMap* tm, const void* base, int dtype,
 
 // Shapes this kernel takes (everything else stays on the mma.sync kernel of attention.cu).
 bool attention_tc_supported(const AttnParams& p) {
+  const int kvb = p.kv_batch_rows ? p.kv_batch_rows : p.Lk;  // TMA row coordinates of K and Q are 32-bit
+  const int qbr = p.q_batch_rows ? p.q_batch_rows : p.Lq;
   auto al = [](const void* q) { return ((uintptr_t)q & 15) == 0; };
   if (!(al(p.q_hi) && al(p.q_lo) && al(p.k_hi) && al(p.k_lo) && al(p.v_hi) && al(p.v_lo) && al(p.o_hi) && al(p.o_lo) && al(p.o_lo8) && al(p.o_hi8)))
     return false;
   return p.D == 32 && p.split != 0 && p.rel_bias == nullptr && p.q_lo && p.k_lo && p.v_lo && (p.ldq % 8 == 0) && (p.ldk % 8 == 0) &&
          (p.ldv % 8 == 0) && (p.ldo % 8 == 0) && (p.o_lo8 == nullptr || p.ldo8 % 8 == 0) && p.H <= 65535 && p.B <= 65535 && p.Lk >= 1 &&
-         p.Lk <= ATC_MAX_LK;
+         (long long)p.B * kvb <= 0x7fffffffll && (long long)p.B * qbr <= 0x7fffffffll;
 }
 
 cudaError_t launch_attention_tc(const AttnParams& p, void* encode_fn, cudaStream_t stream) {

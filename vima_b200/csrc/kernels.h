@@ -68,16 +68,17 @@ __device__ __forceinline__ void attn_store_pair(const AttnParams& p, size_t brow
   }
 }
 constexpr int ATTN_TAIL_MAX_ROWS = 8;         // attention_tail.cu: query rows per (batch, head) the SIMT tail kernel takes
+constexpr int ATTN_TAIL_MAX_LK = 512;         // attention_tail.cu: keys the SIMT tail kernel's shared memory is sized for
 cudaError_t launch_attention(const AttnParams& p, cudaStream_t stream);
 size_t attention_smem_bytes(const AttnParams& p);             // dynamic shared memory the mma.sync kernel needs for p
 int attention_max_lk(const AttnParams& p, size_t smem_limit);  // largest Lk (multiple of 64) that fits smem_limit at p's format
-bool attention_tc_supported(const AttnParams& p);  // wgmma variant (attention_tc.cu): head_dim 32, split operands, no bias, Lk <= 512
+bool attention_tc_supported(const AttnParams& p);  // wgmma variant (attention_tc.cu): head_dim 32, split operands, no bias, K/V streamed (no length cap)
 cudaError_t launch_attention_tc(const AttnParams& p, void* encode_tiled_fn, cudaStream_t stream);  // encode_tiled_fn: cuTensorMapEncodeTiled
 // wgmma variant for the T5 encoder (attention_bias_tc.cu): head_dim 64, relative bias, non-causal, K/V streamed (no length cap)
 bool attention_bias_tc_supported(const AttnParams& p);
 cudaError_t launch_attention_bias_tc(const AttnParams& p, void* encode_tiled_fn, cudaStream_t stream);
-// query rows [row0, row0 + nt) of every (batch, head) (nt <= ATTN_TAIL_MAX_ROWS, head_dim 32, Lk <= 512): the rows that would
-// otherwise occupy a nearly empty 128-row tile of the wgmma kernel
+// query rows [row0, row0 + nt) of every (batch, head) (nt <= ATTN_TAIL_MAX_ROWS, head_dim 32, Lk <= ATTN_TAIL_MAX_LK): the rows that
+// would otherwise occupy a nearly empty 128-row tile of the wgmma kernel
 cudaError_t launch_attention_tail(const AttnParams& p, int row0, int nt, cudaStream_t stream);
 
 struct SmallAttnParams {  // tiny-sequence fp32 attention (ViT: 5 tokens, 24 heads of 32)
