@@ -1,20 +1,16 @@
-"""Prompts past the resident-K/V attention kernel's 384 keys: the T5 encoder on the K/V-streaming wgmma kernel (attention_bias_tc.cu).
+"""Prompts past the resident-K/V attention kernel's 384 keys: the T5 encoder on the K/V-streaming wgmma kernel (attention_tc.cu,
+attention_bias_tc_kernel).
 
 CPU:
   * the oracle's T5 encoder and VIMAPolicy chain against tests/golden/long_prompt.npz (minted from the unmodified reference by
     tests/golden/make_long_prompt_golden.py): a 512-position policy with a 512-token and a ragged 483-token prompt, and T5 alone at
-    Lp = 1000;
-  * what ptxas makes of attention_bias_tc.cu: no serialised wgmma, no spill, M64 N64 K16 instructions in the SASS.
+    Lp = 1000.
+  (What ptxas makes of the kernel is checked in tests/test_wgmma_ptxas_cpu.py.)
 GPU:
   * the kernel against one fp64 statement of T5 attention in every operand and output format, at every chunk boundary up to 2048 keys,
     with attn_bias=tc and with the default options; the defaults leave every shape the resident kernel takes on that kernel, bit for bit;
   * vnn.T5PromptEncoder at Lp = 512 and 1000 against the golden and the oracle, and the 512-position VIMAPolicy chain against the golden.
 """
-import os
-import re
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
@@ -95,40 +91,6 @@ def test_oracle_policy_matches_long_prompt_golden():
     for k, v in modes.items():
         e, a = golden_pick(g, f"policy.mode.{k}", v)
         assert np.array_equal(e, a), k
-
-
-# ------------------------------------------------------------------------------------------------------------------------------
-# ptxas (CPU)
-# ------------------------------------------------------------------------------------------------------------------------------
-def test_attention_bias_tc_ptxas():
-    """attention_bias_tc.cu compiled as the library build compiles it, plus -Xptxas -v: no wgmma serialisation warning (C7510 /
-    C7520), no spill in any instantiation, and M64 N64 K16 wgmmas (fp16 and bf16) in the SASS."""
-    from tests.test_wgmma_ptxas_cpu import _functions, _tool
-    from vima_b200 import build as vbuild
-
-    nvcc = _tool("nvcc")
-    if nvcc is None:
-        pytest.skip("nvcc not found")
-    tmp = tempfile.mkdtemp(prefix="vima_ptxas_bias_")
-    try:
-        obj = os.path.join(tmp, "attention_bias_tc.o")
-        r = subprocess.run([nvcc, *vbuild.NVCC_FLAGS, "-Xptxas", "-v", "-c", os.path.join(vbuild.CSRC, "attention_bias_tc.cu"), "-o", obj],
-                           capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr[-4000:]
-        log = r.stderr
-        bad = [ln.strip() for ln in log.splitlines() if re.search(r"C75[12]0|wgmma\.mma_async instructions are serialized", ln)]
-        assert not bad, "\n".join(bad)
-        fns = {k: v for k, v in _functions(log).items() if "attention_bias_tc_kernel" in k}
-        assert len(fns) == 4, fns  # {f16, bf16} x {split, single-pass}
-        spilled = {k: v for k, v in fns.items() if v != (0, 0)}
-        assert not spilled, spilled
-        cuobjdump = _tool("cuobjdump")
-        if cuobjdump:
-            sass = subprocess.run([cuobjdump, "-sass", obj], capture_output=True, text=True, check=True).stdout
-            assert re.search(r"HGMMA\.64x64x16\.F32(?!\.BF16)", sass)
-            assert re.search(r"HGMMA\.64x64x16\.F32\.BF16", sass)
-    finally:
-        shutil.rmtree(tmp, ignore_errors=True)
 
 
 # ------------------------------------------------------------------------------------------------------------------------------

@@ -3,11 +3,12 @@
 The GEMM and attention main loops only reach the tensor-core rate if ptxas keeps the wgmma pipeline asynchronous: a wgmma
 under a run-time branch or a function call in the loop makes it serialise every wgmma of the kernel ("Potential Performance
 Loss: wgmma.mma_async instructions are serialized"), and accumulators spilled to local memory stall it.  This compiles the
-GEMM instantiation sources and the attention kernel exactly as vima_b200/build.py does, plus -Xptxas -v, and checks
+GEMM instantiation sources and the streaming attention kernel (attention_tc.cu) exactly as vima_b200/build.py does, plus
+-Xptxas -v, and checks
 
-  * no serialisation warning for gemm_tc_kernel or attention_tc_kernel,
-  * no spill bytes in any epilogue-specialised gemm_tc_kernel (the generic runtime-flag variant is exempt),
-  * the full-width instructions (64x128 fp16 and e4m3) are in the SASS.
+  * no serialisation warning for gemm_tc_kernel or any attention instantiation,
+  * no spill bytes in any epilogue-specialised gemm_tc_kernel (the generic runtime-flag variant is exempt) or attention instantiation,
+  * the full-width instructions (64x128 fp16 and e4m3; attention's 64x64 and 64x32) are in the SASS.
 
 About 35 s on 8 cores (the sources compile in parallel, like the library build).
 """
@@ -52,7 +53,7 @@ def compiled():
         sass = {}
         cuobjdump = _tool("cuobjdump")
         for src, obj, _ in results:
-            if src in ("gemm_tc_f16.cu", "gemm_tc_f16f8.cu") and cuobjdump:
+            if src in ("gemm_tc_f16.cu", "gemm_tc_f16f8.cu", "attention_tc.cu") and cuobjdump:
                 sass[src] = subprocess.run([cuobjdump, "-sass", obj], capture_output=True, text=True, check=True).stdout
         yield {src: log for src, _, log in results}, sass
     finally:
@@ -97,3 +98,25 @@ def test_full_width_wgmma_in_sass(compiled):
     assert re.search(r"HGMMA\.64x128x16\.F32", sass["gemm_tc_f16.cu"])
     assert re.search(r"QGMMA\.64x128x32\.F32\.E4M3\.E4M3", sass["gemm_tc_f16f8.cu"])
     assert re.search(r"HGMMA\.64x128x16\.F32", sass["gemm_tc_f16f8.cu"])
+
+
+def test_attention_tc_ptxas(compiled):
+    """The one streaming attention body's six instantiations: the decoder entry point (attention_tc_kernel, f16 and bf16) and the
+    T5 entry point (attention_bias_tc_kernel, {f16, bf16} x {split, single-pass}).  None has a wgmma serialisation warning (C7510 /
+    C7520) or spills; the SASS has the M64 N64 K16 wgmmas (QK^T, and PV at head_dim 64) in fp16 and bf16 and the decoder's
+    M64 N32 K16 PV wgmma."""
+    logs, sass = compiled
+    log = logs["attention_tc.cu"]
+    bad = [ln.strip() for ln in log.splitlines() if re.search(r"C75[12]0|wgmma\.mma_async instructions are serialized", ln)]
+    assert not bad, "\n".join(bad)
+    fns = _functions(log)
+    decoder = {k: v for k, v in fns.items() if "attention_tc_kernel" in k}
+    t5 = {k: v for k, v in fns.items() if "attention_bias_tc_kernel" in k}
+    assert len(decoder) == 2 and len(t5) == 4 and len(fns) == 6, fns
+    spilled = {k: v for k, v in fns.items() if v != (0, 0)}
+    assert not spilled, spilled
+    if "attention_tc.cu" not in sass:
+        pytest.skip("cuobjdump not found")
+    assert re.search(r"HGMMA\.64x64x16\.F32(?!\.BF16)", sass["attention_tc.cu"])
+    assert re.search(r"HGMMA\.64x64x16\.F32\.BF16", sass["attention_tc.cu"])
+    assert re.search(r"HGMMA\.64x32x16\.F32", sass["attention_tc.cu"])

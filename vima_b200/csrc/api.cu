@@ -19,7 +19,6 @@ struct vima_ctx {
   long long launches;
   char err[512];
   void* encode_tiled;  // cuTensorMapEncodeTiled
-  bool gemm_attr_set;
   // environment, read once in vima_create
   int attn_tc;       // VIMA_B200_ATTN: tc (1, default) | mma (0)
   int attn_tail;     // VIMA_B200_ATTN_TAIL: the <= 8 rows past the last full 128-row tile: 1 = "kernel" (default; SIMT tail kernel),
@@ -44,10 +43,6 @@ struct DeviceGuard {
     if (armed) cudaSetDevice(prev);
   }
 };
-
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
 static int fail(vima_ctx* c, int code, const char* fmt, ...) {
   if (c) {
@@ -207,26 +202,17 @@ int vima_row_stats_finalize(vima_ctx* c, const float* partial, int64_t rows, int
 
 // fp8 operand tile: rows of 64 bytes (64 K-elements), 64-byte swizzle
 static int make_tmap_f8(vima_ctx* c, CUtensorMap* tm, const void* base, int rows, int cols, int ld, int box_rows) {
-  const cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  const cuuint64_t gstride[1] = {(cuuint64_t)ld};
-  const cuuint32_t box[2] = {(cuuint32_t)GEMM_BK, (cuuint32_t)box_rows};
-  const cuuint32_t estr[2] = {1, 1};
-  CUresult r = ((PFN_encodeTiled)c->encode_tiled)(tm, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(base), gdim, gstride, box, estr,
-                                                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                                                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = encode_tmap_2d(c->encode_tiled, tm, CU_TENSOR_MAP_DATA_TYPE_UINT8, base, (uint64_t)rows, (uint64_t)cols, (uint64_t)ld, GEMM_BK,
+                              (uint32_t)box_rows, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
   if (r != CUDA_SUCCESS) return fail(c, VIMA_E_CUDA, "cuTensorMapEncodeTiled(fp8) failed (%d): rows %d cols %d ld %d box %d", (int)r, rows, cols, ld, box_rows);
   return VIMA_OK;
 }
 
+// 16-bit operand tile: rows of 128 bytes (64 K-elements), 128-byte swizzle
 static int make_tmap(vima_ctx* c, CUtensorMap* tm, const void* base, int dtype, int rows, int cols, int ld, int box_rows) {
-  const cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  const cuuint64_t gstride[1] = {(cuuint64_t)ld * 2};
-  const cuuint32_t box[2] = {(cuuint32_t)GEMM_BK, (cuuint32_t)box_rows};
-  const cuuint32_t estr[2] = {1, 1};
   const CUtensorMapDataType dt = dtype == DT_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  CUresult r = ((PFN_encodeTiled)c->encode_tiled)(tm, dt, 2, const_cast<void*>(base), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                                                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  CUresult r = encode_tmap_2d(c->encode_tiled, tm, dt, base, (uint64_t)rows, (uint64_t)cols, (uint64_t)ld * 2, GEMM_BK, (uint32_t)box_rows,
+                              CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
   if (r != CUDA_SUCCESS) return fail(c, VIMA_E_CUDA, "cuTensorMapEncodeTiled failed (%d): rows %d cols %d ld %d box %d", (int)r, rows, cols, ld, box_rows);
   return VIMA_OK;
 }
@@ -320,7 +306,7 @@ int vima_gemm(vima_ctx* c, const vima_gemm_desc* d_in, void* stream) {
   GemmLaunch l;
   l.act = d->act; l.glu = d->glu != 0; l.mul = d->mul != nullptr; l.res = d->residual != nullptr;
   l.o32 = d->out_f32 != nullptr; l.o16 = d->out_hi != nullptr; l.dtype = d->dtype;
-  l.lna = d->row_stats != nullptr; l.lnr = d->res_stats != nullptr; l.stats = d->stats_out != nullptr; l.device = c->device;
+  l.lna = d->row_stats != nullptr; l.lnr = d->res_stats != nullptr; l.stats = d->stats_out != nullptr;
   l.split = split; l.block_n = bn;
   // f16f8 (split 2) is fp16-only (checked above)
   auto launch = d->dtype == DT_BF16 ? (split ? launch_gemm_tc<DT_BF16, 1> : launch_gemm_tc<DT_BF16, 0>)
@@ -426,7 +412,7 @@ int vima_attention(vima_ctx* c, const vima_attn_desc* d_in, void* stream) {
   // T5's relative-bias attention (head_dim 64, non-causal): the streaming wgmma kernel takes every length the resident-K/V kernel
   // cannot hold, and every length with attn_bias=tc.  Everything that fits stays on the mma.sync kernel below by default.
   if (c->attn_tc && attention_bias_tc_supported(p) && (c->attn_bias_tc || attention_smem_bytes(p) > (size_t)c->max_smem_optin))
-    LAUNCHED(c, launch_attention_bias_tc(p, c->encode_tiled, (cudaStream_t)stream), "attention_bias_tc");
+    LAUNCHED(c, launch_attention_tc(p, c->encode_tiled, (cudaStream_t)stream), "attention_bias_tc");
   {
     // the mma.sync kernel keeps K and V^T (hi + lo) of one (batch, head) resident in shared memory
     const size_t need = attention_smem_bytes(p);

@@ -14,9 +14,6 @@
 
 namespace vima {
 
-constexpr float FP32_MIN = -3.4028234663852886e38f;
-constexpr float LOG2E = 1.4426950408889634f;
-
 template <int DT>
 __device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
   if constexpr (DT == DT_F16) {
@@ -39,12 +36,7 @@ __device__ __forceinline__ void ldmatrix_x4(uint32_t (&r)[4], const void* smem_r
                : "r"(smem_u32(smem_row_ptr)));
 }
 
-// Scores are kept in the log2 domain: y = s * (scale*log2e) [+ bias*log2e]; the soft causal constant becomes
-// -1e4*log2e; the key-mask constant stays finfo.min (any value + finfo.min rounds to finfo.min, so "all masked keys are
-// equal" -- the reference's degenerate uniform row -- is preserved). softmax is invariant to the common factor.
-constexpr float CAUSAL_L2 = -1e4f * LOG2E;
-constexpr float EXIT_L2 = -9000.f * LOG2E;
-
+// Scores are kept in the log2 domain (kernels.h: FP32_MIN, CAUSAL_L2, EXIT_L2).
 template <int D, int DT, bool SPLIT>
 __global__ void __launch_bounds__(256, (D == 32) ? 2 : 1) attention_kernel(const AttnParams p) {
   constexpr int KS = D / 16;   // k-steps over head_dim for Q K^T
@@ -96,11 +88,7 @@ __global__ void __launch_bounds__(256, (D == 32) ? 2 : 1) attention_kernel(const
       if (SPLIT) Vt_lo[(c * 8 + e) * VROW + j] = vls[e];
     }
   }
-  for (int j = tid; j < Lk_pad; j += 256) {
-    float m = -INFINITY;  // beyond the sequence: excluded
-    if (j < Lk) m = (p.key_mask == nullptr || p.key_mask[(size_t)b * mld + j]) ? 0.f : FP32_MIN;
-    maskadd[j] = m;
-  }
+  for (int j = tid; j < Lk_pad; j += 256) maskadd[j] = attn_key_mask_term(p, b, mld, j, Lk);
   if (p.rel_bias)
     for (int j = tid; j < 2 * Lk - 1; j += 256) sbias[j] = __ldg(p.rel_bias + (size_t)h * (2 * Lk - 1) + j) * LOG2E;
   if (tid == 0) *qb_counter = 0;
@@ -282,26 +270,12 @@ __global__ void __launch_bounds__(256, (D == 32) ? 2 : 1) attention_kernel(const
     const float inv0 = 1.0f / lrow[0], inv1 = 1.0f / lrow[1];
 #pragma unroll
     for (int n = 0; n < ND; ++n) {
-      const int c = h * D + n * 8 + 2 * t;
-      uint32_t hi, lo;
 #pragma unroll
       for (int half = 0; half < 2; ++half) {
         const int r = half ? r1 : r0;
         if (r >= Lq) continue;
-        const float x0 = o[n][2 * half] * (half ? inv1 : inv0), x1 = o[n][2 * half + 1] * (half ? inv1 : inv0);
-        pack_split<DT>(x0, x1, hi, lo);
-        const size_t off = ((size_t)b * qbr + r) * p.ldo + c;
-        *reinterpret_cast<uint32_t*>(p.o_hi + off) = hi;
-        if (p.o_lo) *reinterpret_cast<uint32_t*>(p.o_lo + off) = lo;
-        if (p.o_lo8) {  // e4m3 cross-term views for an "f16f8" consumer GEMM
-          const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hi));
-          unsigned short l8, h8;
-          asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(l8) : "f"((x1 - hf.y) * F8_ACT_LO_SCALE), "f"((x0 - hf.x) * F8_ACT_LO_SCALE));
-          asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(h8) : "f"(x1 * F8_ACT_HI_SCALE), "f"(x0 * F8_ACT_HI_SCALE));
-          const size_t off8 = ((size_t)b * qbr + r) * p.ldo8 + c;
-          *reinterpret_cast<unsigned short*>(p.o_lo8 + off8) = l8;
-          *reinterpret_cast<unsigned short*>(p.o_hi8 + off8) = h8;
-        }
+        const float inv = half ? inv1 : inv0;
+        attn_store_pair<DT>(p, (size_t)b * qbr + r, h * D + n * 8 + 2 * t, o[n][2 * half] * inv, o[n][2 * half + 1] * inv);
       }
     }
   }
@@ -330,19 +304,10 @@ int attention_max_lk(const AttnParams& p, size_t smem_limit) {
 template <int D, int DT, bool SPLIT>
 static cudaError_t launch_attn_t(const AttnParams& p, cudaStream_t stream) {
   const size_t smem = attention_smem_bytes(p);
-  auto kern = attention_kernel<D, DT, SPLIT>;
-  // the opt-in shared-memory ceiling is set once per (instantiation, device): not a stream operation, and not legal inside a
-  // CUDA-graph capture, so it must not ride on every launch
-  static int attr_smem[64] = {};
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if ((int)smem > attr_smem[dev & 63]) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    attr_smem[dev & 63] = (int)smem;
-  }
+  const cudaError_t e = raise_smem_ceiling<attention_kernel<D, DT, SPLIT>>((int)smem);  // raised to the largest Lk seen so far
+  if (e != cudaSuccess) return e;
   dim3 grid(p.H, p.B);
-  kern<<<grid, 256, smem, stream>>>(p);
+  attention_kernel<D, DT, SPLIT><<<grid, 256, smem, stream>>>(p);
   return cudaGetLastError();
 }
 

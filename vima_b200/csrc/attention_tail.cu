@@ -22,9 +22,6 @@ namespace {
 constexpr int TAIL_NT = ATTN_TAIL_MAX_ROWS;
 constexpr int TAIL_WARPS = 8;
 constexpr int TAIL_D = 32;
-constexpr float FP32_MIN_TL = -3.4028234663852886e38f;
-constexpr float LOG2E_TL = 1.4426950408889634f;
-constexpr float CAUSAL_L2_TL = -1e4f * LOG2E_TL;
 
 template <int DT>
 __device__ __forceinline__ float2 unpack2(uint32_t w) {
@@ -65,7 +62,7 @@ __global__ void __launch_bounds__(TAIL_WARPS * 32) attention_tail_kernel(const A
   lk_pad = (Lk + 31) & ~31;  // keys this batch element walks (the shared-memory carve above keeps the launch's capacity)
 
   // ---- queries: lane = dim ----
-  const float c_l2 = p.scale * LOG2E_TL;
+  const float c_l2 = p.scale * LOG2E;
 #pragma unroll
   for (int i = 0; i < TAIL_NT; ++i) {
     float q = 0.f;
@@ -117,8 +114,9 @@ __global__ void __launch_bounds__(TAIL_WARPS * 32) attention_tail_kernel(const A
       }
     }
     if (j0 + 32 < lk_pad) load_k(j + 32);
-    float madd = -INFINITY;  // beyond the sequence: excluded
-    if (valid) madd = (p.key_mask == nullptr || p.key_mask[(size_t)b * mld + j]) ? 0.f : FP32_MIN_TL;
+    // attn_key_mask_term(p, b, mld, j, Lk) written out: through the helper, ptxas gives this kernel 3 to 5 more registers
+    float madd = -INFINITY;
+    if (valid) madd = (p.key_mask == nullptr || p.key_mask[(size_t)b * mld + j]) ? 0.f : FP32_MIN;
     float y[TAIL_NT];
 #pragma unroll
     for (int i = 0; i < TAIL_NT; ++i) {
@@ -132,7 +130,7 @@ __global__ void __launch_bounds__(TAIL_WARPS * 32) attention_tail_kernel(const A
       }
       const float2 s0 = unpack64(a0), s1 = unpack64(a1);
       float v = ((s0.x + s0.y) + (s1.x + s1.y)) + madd;
-      if (p.causal && j > pos0 + i) v = CAUSAL_L2_TL + madd;
+      if (p.causal && j > pos0 + i) v = CAUSAL_L2 + madd;
       y[i] = v;
       mx[i] = fmaxf(mx[i], v);
     }
@@ -243,16 +241,11 @@ cudaError_t launch_attention_tail(const AttnParams& p, int row0, int nt, cudaStr
   const size_t smem = (size_t)TAIL_WARPS * (TAIL_NT * TAIL_D + (size_t)lk_pad * TAIL_NT) * sizeof(float);
   constexpr size_t smem_max = (size_t)TAIL_WARPS * (TAIL_NT * TAIL_D + (size_t)ATTN_TAIL_MAX_LK * TAIL_NT) * sizeof(float);
   if (smem > smem_max) return cudaErrorInvalidValue;
-  static bool attr_set[2][64] = {};  // once per (format, device): not legal inside a CUDA-graph capture
-  int dev = 0;
-  cudaGetDevice(&dev);
   const int fi = p.dtype == DT_BF16 ? 1 : 0;
-  if (!attr_set[fi][dev & 63]) {
-    cudaError_t e = fi ? cudaFuncSetAttribute(attention_tail_kernel<DT_BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max)
-                       : cudaFuncSetAttribute(attention_tail_kernel<DT_F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max);
-    if (e != cudaSuccess) return e;
-    attr_set[fi][dev & 63] = true;
-  }
+  // the ceiling is the capacity's, so it is set once, whatever Lk the first call has
+  const cudaError_t e = fi ? raise_smem_ceiling<attention_tail_kernel<DT_BF16>>((int)smem_max)
+                           : raise_smem_ceiling<attention_tail_kernel<DT_F16>>((int)smem_max);
+  if (e != cudaSuccess) return e;
   const long long units = (long long)p.B * p.H;
   const unsigned grid = (unsigned)((units + TAIL_WARPS - 1) / TAIL_WARPS);
   if (fi) attention_tail_kernel<DT_BF16><<<grid, TAIL_WARPS * 32, smem, stream>>>(p, row0, nt, lk_pad);

@@ -270,35 +270,60 @@ template <int R>
 __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 template <int R>
 __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
-// A from registers (the 16-bit fragment of a previous accumulator), B K-major in shared memory: M64 N32 K16
-template <int DT>
-__device__ __forceinline__ void wgmma_m64n32k16_rs(float (&d)[16], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
-  if constexpr (DT == DT_F16) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 " VIMA_R16 ", {%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}"
-                 : VIMA_ACC16(d) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
-  } else {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 " VIMA_R16 ", {%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}"
-                 : VIMA_ACC16(d) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
-  }
+// A from registers (the 16-bit fragment of a previous accumulator), B K-major in shared memory: M64 N{N} K16 (attention's
+// O[64 x D] += P V).  IA / IB / IP as above.
+#define VIMA_WGMMA_K16_RS(N, R, ACC, IA, IB, IP)                                                                                   \
+  if constexpr (DT == DT_F16)                                                                                                      \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, " IP ", 0;\n\t"                                                             \
+                 "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32.f16.f16 " R ", " IA ", " IB ", p, 1, 1, 0;\n\t}"                 \
+                 : ACC(d) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));                               \
+  else                                                                                                                             \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, " IP ", 0;\n\t"                                                             \
+                 "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32.bf16.bf16 " R ", " IA ", " IB ", p, 1, 1, 0;\n\t}"               \
+                 : ACC(d) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate))
+template <int DT, int N>
+__device__ __forceinline__ void wgmma_m64nNk16_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+  static_assert(N == 32 || N == 64, "wgmma_m64nNk16_rs: N is 32 or 64");
+  if constexpr (N == 32) { VIMA_WGMMA_K16_RS(32, VIMA_R16, VIMA_ACC16, "{%16, %17, %18, %19}", "%20", "%21"); }
+  else { VIMA_WGMMA_K16_RS(64, VIMA_R32, VIMA_ACC32, "{%32, %33, %34, %35}", "%36", "%37"); }
 }
-// the same with N64 (head_dim 64 attention: O[64 x 64] += P V)
-template <int DT>
-__device__ __forceinline__ void wgmma_m64n64k16_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
-  if constexpr (DT == DT_F16) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 " VIMA_R32 ", {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
-                 : VIMA_ACC32(d) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
-  } else {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
-                 "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 " VIMA_R32 ", {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
-                 : VIMA_ACC32(d) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
-  }
-}
+#undef VIMA_WGMMA_K16_RS
 
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+
+// ---------------------------------------------------------------------------------------------
+// host-side launch helpers
+// ---------------------------------------------------------------------------------------------
+// 2-D tiled TMA map of a row-major [rows, cols] matrix (row pitch ld_bytes), boxes of box_cols x box_rows elements.
+// encode_fn is the driver's cuTensorMapEncodeTiled (cudaGetDriverEntryPoint; the runtime links no libcuda).
+inline CUresult encode_tmap_2d(void* encode_fn, CUtensorMap* tm, CUtensorMapDataType dtype, const void* base, uint64_t rows, uint64_t cols,
+                               uint64_t ld_bytes, uint32_t box_cols, uint32_t box_rows, CUtensorMapSwizzle swizzle,
+                               CUtensorMapL2promotion l2_promotion) {
+  typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                      const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                      CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+  const cuuint64_t gdim[2] = {cols, rows};
+  const cuuint64_t gstride[1] = {ld_bytes};
+  const cuuint32_t box[2] = {box_cols, box_rows};
+  const cuuint32_t estr[2] = {1, 1};
+  return ((PFN_encodeTiled)encode_fn)(tm, dtype, 2, const_cast<void*>(base), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
+                                      l2_promotion, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+}
+
+// Raises KERNEL's dynamic shared-memory ceiling on the current device to at least `bytes`.  cudaFuncSetAttribute is no stream
+// operation and is not legal inside a CUDA-graph capture, so the ceiling only ever grows and is set once per (instantiation,
+// device) for a fixed size: after the first launch a capture never sees the call.
+template <auto KERNEL>
+inline cudaError_t raise_smem_ceiling(int bytes) {
+  static int ceiling[64] = {};  // per device (function attributes are per device)
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (bytes <= ceiling[dev & 63]) return cudaSuccess;
+  const cudaError_t e = cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e == cudaSuccess) ceiling[dev & 63] = bytes;
+  return e;
 }
 
 }  // namespace vima

@@ -10,7 +10,6 @@ struct GemmLaunch {
   int act, glu, mul, res, o32, o16, dtype;
   int lna, lnr, stats;  // folded A-side LayerNorm, LayerNorm'd residual, partial row statistics of the output
   int split, block_n;   // kernel template parameters: split mode (0 / 1 / 2) and tile width (32, 64, 96, 128)
-  int device;           // function attributes are per device
 };
 
 // (ACT, GLU, MUL, RES, O32, O16, DT, LNA, LNR, STATS)
@@ -30,14 +29,9 @@ struct GemmLaunch {
   X(ACT_NONE, false, false, false, true, false, DT, true, false, false)       /* ViT in_proj with ln_1 folded in -> fp32 */
 
 template <class E, int SPLIT, int BN>
-inline cudaError_t launch_one(const GemmParams& p, int grid, size_t smem, int max_smem, cudaStream_t stream, int device) {
-  static bool attr_set[64] = {};  // per instantiation and device (function attributes are per device)
-  const int di = device & 63;
-  if (!attr_set[di]) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<E, SPLIT, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);
-    if (e != cudaSuccess) return e;
-    attr_set[di] = true;
-  }
+inline cudaError_t launch_one(const GemmParams& p, int grid, size_t smem, int max_smem, cudaStream_t stream) {
+  const cudaError_t e = raise_smem_ceiling<gemm_tc_kernel<E, SPLIT, BN>>(max_smem);  // the device's opt-in limit: set once
+  if (e != cudaSuccess) return e;
   gemm_tc_kernel<E, SPLIT, BN><<<grid, GEMM_THREADS, smem, stream>>>(p);
   return cudaGetLastError();
 }
@@ -45,11 +39,11 @@ inline cudaError_t launch_one(const GemmParams& p, int grid, size_t smem, int ma
 // GLU tiles are 64 or 128 columns wide (a value and a gate half of 32-column multiples); other tiles 32, 64, 96 or 128
 template <class E, int SPLIT>
 inline cudaError_t launch_bn(const GemmParams& p, const GemmLaunch& l, int grid, size_t smem, int max_smem, cudaStream_t stream) {
-  if (l.block_n == 64) return launch_one<E, SPLIT, 64>(p, grid, smem, max_smem, stream, l.device);
-  if (l.block_n == 128) return launch_one<E, SPLIT, 128>(p, grid, smem, max_smem, stream, l.device);
+  if (l.block_n == 64) return launch_one<E, SPLIT, 64>(p, grid, smem, max_smem, stream);
+  if (l.block_n == 128) return launch_one<E, SPLIT, 128>(p, grid, smem, max_smem, stream);
   if constexpr (E::GENERIC || !E::GLU) {
-    if (l.block_n == 32) return launch_one<E, SPLIT, 32>(p, grid, smem, max_smem, stream, l.device);
-    if (l.block_n == 96) return launch_one<E, SPLIT, 96>(p, grid, smem, max_smem, stream, l.device);
+    if (l.block_n == 32) return launch_one<E, SPLIT, 32>(p, grid, smem, max_smem, stream);
+    if (l.block_n == 96) return launch_one<E, SPLIT, 96>(p, grid, smem, max_smem, stream);
   }
   return cudaErrorInvalidValue;
 }

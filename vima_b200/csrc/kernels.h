@@ -37,6 +37,19 @@ struct AttnParams {
   int q_batch_rows;                            // rows between consecutive batch elements in q / o (>= Lq), 0 = Lq
   const int* q_pos;                            // causal, per batch element (device, or null): position q_pos[b], keys q_pos[b] + Lq
 };
+// Attention scores are kept in the log2 domain: y = s * (scale*log2e) [+ bias*log2e]; the soft causal constant becomes
+// -1e4*log2e; the key-mask constant stays finfo.min (any value + finfo.min rounds to finfo.min, so "all masked keys are
+// equal" -- the reference's degenerate uniform row -- is preserved). softmax is invariant to the common factor.
+constexpr float FP32_MIN = -3.4028234663852886e38f;
+constexpr float LOG2E = 1.4426950408889634f;
+constexpr float CAUSAL_L2 = -1e4f * LOG2E;
+constexpr float EXIT_L2 = -9000.f * LOG2E;  // a running row maximum at or below this has only seen hidden or padded keys
+// Additive key-mask term of key j in batch element b (mask row pitch mld): 0 = attend, finfo.min = padded, -inf = past Lk.
+__device__ __forceinline__ float attn_key_mask_term(const AttnParams& p, int b, int mld, int j, int Lk) {
+  float m = -INFINITY;  // beyond the sequence: excluded
+  if (j < Lk) m = (p.key_mask == nullptr || p.key_mask[(size_t)b * mld + j]) ? 0.f : FP32_MIN;
+  return m;
+}
 // Causal position of query row 0 and key count of batch element b.  With q_pos the key count is q_pos[b] + (full query count of the
 // call; q_batch_rows when a body / tail split gave this launch only part of the rows), clamped to the capacity Lk.
 __device__ __forceinline__ void attn_batch_keys(const AttnParams& p, int b, int qbr, int& qp0, int& lk) {
@@ -48,8 +61,8 @@ __device__ __forceinline__ void attn_batch_keys(const AttnParams& p, int b, int 
     lk = max(min(qp0 + qbr, p.Lk), 1);
   }
 }
-// two adjacent output values of one query row (the wgmma attention kernels): (hi, lo) 16-bit pairs [+ e4m3 cross-term views for an
-// "f16f8" consumer GEMM]
+// two adjacent output values of one query row (the tensor-core attention kernels): (hi, lo) 16-bit pairs [+ e4m3 cross-term views for
+// an "f16f8" consumer GEMM]
 template <int DT>
 __device__ __forceinline__ void attn_store_pair(const AttnParams& p, size_t brow, int col, float x0, float x1) {
   uint32_t hi, lo;
@@ -72,11 +85,11 @@ constexpr int ATTN_TAIL_MAX_LK = 512;         // attention_tail.cu: keys the SIM
 cudaError_t launch_attention(const AttnParams& p, cudaStream_t stream);
 size_t attention_smem_bytes(const AttnParams& p);             // dynamic shared memory the mma.sync kernel needs for p
 int attention_max_lk(const AttnParams& p, size_t smem_limit);  // largest Lk (multiple of 64) that fits smem_limit at p's format
-bool attention_tc_supported(const AttnParams& p);  // wgmma variant (attention_tc.cu): head_dim 32, split operands, no bias, K/V streamed (no length cap)
-cudaError_t launch_attention_tc(const AttnParams& p, void* encode_tiled_fn, cudaStream_t stream);  // encode_tiled_fn: cuTensorMapEncodeTiled
-// wgmma variant for the T5 encoder (attention_bias_tc.cu): head_dim 64, relative bias, non-causal, K/V streamed (no length cap)
-bool attention_bias_tc_supported(const AttnParams& p);
-cudaError_t launch_attention_bias_tc(const AttnParams& p, void* encode_tiled_fn, cudaStream_t stream);
+// K/V-streaming wgmma kernel (attention_tc.cu, no length cap), one body with two entry points:
+bool attention_tc_supported(const AttnParams& p);       // the decoders: head_dim 32, split operands, no bias
+bool attention_bias_tc_supported(const AttnParams& p);  // the T5 encoder: head_dim 64, relative bias, non-causal
+// runs p on the entry point its relative bias selects (p must pass one of the two predicates); encode_tiled_fn: cuTensorMapEncodeTiled
+cudaError_t launch_attention_tc(const AttnParams& p, void* encode_tiled_fn, cudaStream_t stream);
 // query rows [row0, row0 + nt) of every (batch, head) (nt <= ATTN_TAIL_MAX_ROWS, head_dim 32, Lk <= ATTN_TAIL_MAX_LK): the rows that
 // would otherwise occupy a nearly empty 128-row tile of the wgmma kernel
 cudaError_t launch_attention_tail(const AttnParams& p, int row0, int nt, cudaStream_t stream);
