@@ -3,10 +3,10 @@ import os
 
 import torch
 
-from .engine import get_precision, set_precision
+from .engine import get_precision, refresh_weights, set_precision
 from .policy import VIMAFlamingoPolicy, VIMAGatoPolicy, VIMAGPTPolicy, VIMAPolicy
 
-__all__ = ["VIMAPolicy", "VIMAGatoPolicy", "VIMAGPTPolicy", "VIMAFlamingoPolicy", "create_policy_from_ckpt", "set_precision", "get_precision"]
+__all__ = ["VIMAPolicy", "VIMAGatoPolicy", "VIMAGPTPolicy", "VIMAFlamingoPolicy", "create_policy_from_ckpt", "set_precision", "get_precision", "refresh_weights"]
 
 
 def create_policy_from_ckpt(ckpt_path, device):

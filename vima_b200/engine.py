@@ -12,7 +12,9 @@ Accumulation, softmax, LayerNorm, residuals and biases are fp32 in every mode.
 """
 from __future__ import annotations
 
+import contextlib
 import math
+import weakref
 from dataclasses import dataclass
 from typing import Dict, Optional, Tuple
 
@@ -211,21 +213,142 @@ def pack_glu(ctx: _C.Context, w_val: torch.Tensor, b_val: Optional[torch.Tensor]
 # packed-weight cache: keyed by the parameters' identity + in-place version, the device and the precision mode
 # -------------------------------------------------------------------------------------------------------------
 class WeightCache:
-    def __init__(self):
+    """Packed weights of one module (`owner`).  An entry is rebuilt when a parameter it was packed from is replaced (new storage:
+    `load_state_dict(assign=True)`, `module.weight = nn.Parameter(...)`, `param.data = t`), written in place through autograd
+    (`load_state_dict`, `copy_` / `mul_` under no_grad: the version counter moves), moved to another device, or when the precision
+    mode changes.  A write through `param.data` (`param.data.copy_(t)`) moves no version counter and is not seen: call
+    `refresh_weights(module)` after one.  `generation` counts the clears, so a captured graph or an open decode cache can tell."""
+
+    def __init__(self, owner: Optional[torch.nn.Module] = None):
         self._store: Dict[str, Tuple[tuple, object]] = {}
+        self._owner = None if owner is None else weakref.ref(owner)  # weak: no module <-> cache reference cycle
+        self.generation = 0
+
+    @property
+    def owner(self) -> Optional[torch.nn.Module]:
+        return None if self._owner is None else self._owner()
 
     def get(self, name: str, params: Tuple[Optional[torch.Tensor], ...], build):
         p = prec()
         key = (p.name,) + tuple((None if t is None else (t.data_ptr(), t._version, str(t.device))) for t in params)
         hit = self._store.get(name)
-        if hit is not None and hit[0] == key:
-            return hit[1]
-        val = build()
-        self._store[name] = (key, val)
+        # the entry also holds weak references to the tensors it was packed from: a replacement that lands in the block its
+        # predecessor freed (same address, same version) is still another tensor
+        if hit is not None and hit[0] == key and all((r is None) if t is None else (r is not None and r() is t) for r, t in zip(hit[2], params)):
+            val = hit[1]
+        else:
+            val = build()
+            self._store[name] = (key, val, tuple(None if t is None else weakref.ref(t) for t in params))
+        if _recorders:
+            _recorders[-1].note(self, params, val)
         return val
 
     def clear(self):
         self._store.clear()
+        self.generation += 1
+
+    def __deepcopy__(self, memo):  # a copied module gets an empty cache owned by the copy
+        owner = self.owner
+        return WeightCache(None if owner is None else memo.get(id(owner), owner))
+
+    def __getstate__(self):  # packed weights and the owner link are not pickled; the unpickled module repacks
+        return {}
+
+    def __setstate__(self, state):
+        self.__init__()
+
+
+def refresh_weights(module: torch.nn.Module) -> None:
+    """Drop every packed weight under `module`; the next call repacks from the parameters as they are.  Needed after a write through
+    `param.data` (which moves no version counter, see WeightCache); graphs captured and decode caches opened before it refuse to run."""
+    for m in module.modules():
+        wc = m.__dict__.get("_wc")
+        if isinstance(wc, WeightCache):
+            wc.clear()
+
+
+def uses(module: torch.nn.Module) -> None:
+    """Called where a module's fp32 parameters go to a kernel without a packed-weight cache (the fp32 grouped GEMMs of the action
+    heads and embeddings, embedding tables, norm gains): while a graph is being captured (`record_weights`), the module becomes one
+    the graph depends on, as the owner of a cache the step used does."""
+    if _recorders:
+        _recorders[-1].note_module(module)
+
+
+class WeightState:
+    """What a captured graph or an open decode cache depends on: the identity, storage and in-place version of every parameter
+    under `modules`, of the (module, name) parameters in `slots` (plus `params` of caches without an owner module) and the clear count of every packed-weight cache there.  It keeps references to those parameters (and to `keep`, the packed
+    weights a graph read), so nothing the device pointers point at is freed while it lives."""
+
+    def __init__(self, modules=(), params=(), keep=(), slots=()):
+        self.precision = prec().name
+        self._slots, self._caches, seen, seen_c = [], [], set(), set()
+        for root in modules:
+            for m in root.modules():
+                wc = m.__dict__.get("_wc")
+                if isinstance(wc, WeightCache) and id(wc) not in seen_c:
+                    seen_c.add(id(wc))
+                    self._caches.append(wc)
+                for n, t in m._parameters.items():
+                    if t is not None and (id(m._parameters), n) not in seen:
+                        seen.add((id(m._parameters), n))
+                        self._slots.append((m._parameters, n, t))
+        for m, n in slots:
+            if (id(m._parameters), n) not in seen:
+                seen.add((id(m._parameters), n))
+                self._slots.append((m._parameters, n, m._parameters[n]))
+        self._loose = tuple(t for t in params if t is not None)
+        self._keep = list(keep)
+        self._fp = self._current()
+
+    def _current(self) -> tuple:
+        return (tuple(c.generation for c in self._caches),
+                tuple((t.data_ptr(), t._version) if d.get(n) is t else None for d, n, t in self._slots),
+                tuple((t.data_ptr(), t._version) for t in self._loose))
+
+    def n_params(self) -> int:
+        return len(self._slots) + len(self._loose)
+
+    def changed(self) -> Optional[str]:
+        """None while every parameter and cache recorded is as it was; otherwise what moved.  (The precision mode is checked by the
+        caller: `precision` holds the one in force when this was taken.)"""
+        if self._current() != self._fp:
+            return "the weights changed (a parameter was replaced, written in place, or refresh_weights was called)"
+        return None
+
+
+class _Recorder:
+    def __init__(self):
+        self.owners, self.params, self.values, self._seen = [], [], [], set()
+
+    def note_module(self, module: torch.nn.Module) -> None:
+        if id(module) not in self._seen:
+            self._seen.add(id(module))
+            self.owners.append(module)
+
+    def note(self, cache: WeightCache, params, val) -> None:
+        self.values.append(val)
+        owner = cache.owner
+        if owner is not None:
+            self.note_module(owner)
+        elif id(cache) not in self._seen:
+            self._seen.add(id(cache))
+            self.params.extend(params)
+
+
+@contextlib.contextmanager
+def record_weights():
+    """Collects every packed-weight cache used inside the block and every module passed to `uses`; yields a callable returning the
+    WeightState of those modules (all their parameters) holding the packed weights used."""
+    rec = _Recorder()
+    _recorders.append(rec)
+    try:
+        yield lambda: WeightState(rec.owners, rec.params, rec.values)
+    finally:
+        _recorders.remove(rec)
+
+
+_recorders: list = []
 
 
 # -------------------------------------------------------------------------------------------------------------

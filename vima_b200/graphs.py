@@ -10,6 +10,12 @@ nothing on the step synchronises with the host after the first call, so the whol
     out = g(new_obs)                                        # copies new_obs into the static inputs, replays
 
 The outputs are the tensors the captured call returned (static storage, overwritten by the next replay).
+
+A graph holds the device pointers of the packed weights and parameters it read, so it is only valid for the weights and the
+precision mode it was captured with.  Capture records them (`engine.record_weights`: every parameter of each module whose packed-
+weight cache the step used) and keeps them alive; each replay first checks them and raises instead of launching when a parameter
+was replaced or written in place, `refresh_weights` was called, or the precision mode changed.  Capture a new graph after a
+weight update.
 """
 from __future__ import annotations
 
@@ -29,6 +35,15 @@ def _map(fn, x, y=None):
     return fn(x) if y is None else fn(x, y)
 
 
+def check_weights(weights: "eng.WeightState", precision: bool = True) -> None:
+    """Raise before a replay that would read stale or freed weights (or run kernels of another precision mode)."""
+    why = weights.changed()
+    if why is None and precision and eng.prec().name != weights.precision:
+        why = f"the precision mode changed from {weights.precision!r} to {eng.prec().name!r}"
+    if why is not None:
+        raise RuntimeError(f"{why} since this CUDA graph was captured; it would replay with the old ones. Capture it again.")
+
+
 class GraphedStep:
     def __init__(self, fn: Callable, example_inputs, *, warmup: int = 3):
         """fn(inputs) -> nest of tensors; `example_inputs`: nest (dict / list / tensor) of CUDA tensors with the step's shapes."""
@@ -45,8 +60,9 @@ class GraphedStep:
         torch.cuda.synchronize(dev)
         self.graph = torch.cuda.CUDAGraph()
         n0 = self.ctx.launches
-        with torch.cuda.graph(self.graph):
+        with eng.record_weights() as weights, torch.cuda.graph(self.graph):
             self.static_out = fn(self.static_in)
+        self.weights = weights()
         self.kernels_per_replay = self.ctx.launches - n0  # vima:: kernels inside the graph (torch's own copies come on top)
         self.replays = 0
 
@@ -62,6 +78,7 @@ class GraphedStep:
             yield x
 
     def __call__(self, inputs):
+        check_weights(self.weights)
         if inputs is not self.static_in:
             _map(lambda dst, src: dst.copy_(src, non_blocking=True) if dst.data_ptr() != src.data_ptr() else dst, self.static_in, inputs)
         self.graph.replay()
@@ -110,8 +127,9 @@ class GraphedSlotStep:
             torch.cuda.synchronize(dev)
             self.graph = torch.cuda.CUDAGraph()
             n0 = self.ctx.launches
-            with torch.cuda.graph(self.graph):
+            with eng.record_weights() as weights, torch.cuda.graph(self.graph):
                 self.static_out = policy._slot_step(cache, *self.static_in)
+            self.weights = weights()
             self.kernels_per_replay = self.ctx.launches - n0
         finally:
             cache.restore(saved)
@@ -121,6 +139,7 @@ class GraphedSlotStep:
     def __call__(self, obs_token: torch.Tensor, *inputs: torch.Tensor) -> torch.Tensor:
         if len(inputs) + 1 != len(self.static_in):
             raise ValueError(f"the graph was captured with {len(self.static_in)} step inputs, got {len(inputs) + 1}")
+        check_weights(self.weights, precision=False)  # the cache refuses another precision mode (ValueError)
         self.cache.check_step(obs_token.shape[1], obs_token.shape[2] if obs_token.dim() == 4 else 1, obs_token.shape[-1], eng.prec())
         if tuple(obs_token.shape) != tuple(self.static_in[0].shape):
             raise ValueError(f"the graph was captured for obs_token {tuple(self.static_in[0].shape)}, got {tuple(obs_token.shape)}")

@@ -169,6 +169,7 @@ class CategoricalNet(nn.Module):
         return [self.mlp], self._dims
 
     def forward(self, x):
+        eng.uses(self)  # fp32 parameters read by the kernels directly
         return ActionDecoder.run_heads([self], x)[0]
 
 
@@ -185,6 +186,7 @@ class MultiCategoricalNet(nn.Module):
         return list(self.mlps), self._dims
 
     def forward(self, x):
+        eng.uses(self)  # fp32 parameters read by the kernels directly
         return ActionDecoder.run_heads([self], x)[0]
 
 
@@ -232,6 +234,7 @@ class ActionDecoder(nn.Module):
 
     def forward(self, x: torch.Tensor):
         """(..., E) -> {key: MultiCategorical}  (action_decoder.py:51-52)."""
+        eng.uses(self)  # fp32 parameters read by the kernels directly
         if not hasattr(self, "_my_grouped"):
             self._my_grouped = _GroupedMLPs()
         keys = list(self._decoders.keys())
@@ -249,6 +252,7 @@ class ContinuousActionEmbedding(nn.Module):
         self.output_dim = output_dim
 
     def forward(self, x: torch.Tensor):
+        eng.uses(self)  # fp32 parameters read by the kernels directly
         if not hasattr(self, "_g"):
             self._g = _GroupedMLPs()
         lead = x.shape[:-1]
@@ -274,6 +278,7 @@ class ActionEmbedding(nn.Module):
 
     def forward(self, x_dict: Dict[str, torch.Tensor]):
         """{key: (..., n_k) float} -> (..., output_dim): per-key MLP, concat in SORTED key order, Linear (:29-37)."""
+        eng.uses(self)  # fp32 parameters read by the kernels directly
         if not self._input_fields_checked:
             assert set(x_dict.keys()) == set(self._embed_dict.keys())
             self._input_fields_checked = True

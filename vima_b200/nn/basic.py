@@ -67,10 +67,11 @@ class Linear(nn.Linear):
 
     def __init__(self, *a, **k):
         super().__init__(*a, **k)
-        self._wc = eng.WeightCache()
+        self._wc = eng.WeightCache(self)
         self._f32 = F32GroupRunner()
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
+        eng.uses(self)  # fp32 parameters read by the kernels directly
         ctx = eng.ctx_for(x)
         p = eng.prec()
         lead = x.shape[:-1]
@@ -103,12 +104,13 @@ class MLPSequential(nn.Sequential):
         return [m for m in self if isinstance(m, nn.Linear)]
 
     def forward(self, x: torch.Tensor, *, want16: bool = False, out16_ld: Optional[int] = None, out16: Optional[eng.Opnd] = None):
+        eng.uses(self)  # fp32 parameters read by the kernels directly
         ctx = eng.ctx_for(x)
         p = eng.prec()
         lins = self._linears()
         want16 = want16 or out16 is not None
         if not hasattr(self, "_wc"):
-            self._wc = eng.WeightCache()
+            self._wc = eng.WeightCache(self)
             self._f32 = [F32GroupRunner() for _ in lins]
         lead = x.shape[:-1]
         cur32: Optional[torch.Tensor] = x.reshape(-1, lins[0].in_features)

@@ -95,7 +95,7 @@ class VisionTransformer(nn.Module):
         self.blocks = nn.Sequential(*[ResidualAttentionBlock(width, heads) for _ in range(layers)])
         self.ln_post = nn.LayerNorm(width)
         self.projection = nn.Parameter(scale * torch.randn(width, output_dim))
-        self._wc = eng.WeightCache()
+        self._wc = eng.WeightCache(self)
 
     def _packed(self, ctx, p):
         def build():
@@ -182,7 +182,7 @@ class ObjEncoder(nn.Module):
                                        for v in views})
         self.pre_transformer_layer = nn.ModuleDict({v: nn.Linear(self.cropped_img_encoder.output_dim + bbox_mlp_hidden_dim, transformer_emb_dim)
                                                     for v in views})
-        self._wc = eng.WeightCache()
+        self._wc = eng.WeightCache(self)
 
     @property
     def output_dim(self):
@@ -303,7 +303,7 @@ class GatoVisionTransformerRectangular(nn.Module):
         self.ln_post = nn.LayerNorm(width)
         self.projection = nn.Parameter(scale * torch.randn(width, output_dim))
         self.img_patch_len = nh * nw
-        self._wc = eng.WeightCache()
+        self._wc = eng.WeightCache(self)
 
     def encode_u8(self, img_u8: torch.Tensor) -> torch.Tensor:
         """(N,3,H,W) uint8 -> (N, n_patches, output_dim) fp32."""

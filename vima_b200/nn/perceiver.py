@@ -87,7 +87,7 @@ class ObjectsPerceiverEncoder(nn.Module):
         self._num_queries = num_latents
         self._num_blocks = num_blocks
         self._heads_self, self._heads_cross = num_self_attention_heads, num_cross_attention_heads
-        self._wc = eng.WeightCache()
+        self._wc = eng.WeightCache(self)
 
     # -------------------------------------------------------------------------------------------------
     def _packed(self, ctx, p):

@@ -113,7 +113,7 @@ class T5PromptEncoder(nn.Module):
         for m in self.modules():
             if isinstance(m, nn.Linear):
                 nn.init.normal_(m.weight, std=m.in_features ** -0.5)
-        self._wc = eng.WeightCache()
+        self._wc = eng.WeightCache(self)
         self._bucket_cache = {}
 
     def _packed(self, ctx, p):

@@ -80,9 +80,10 @@ class DecodeCache:
     causal block appends the new tokens' keys/values to `kv[i]` ([B*Lmax, 2E] (hi, lo) pairs) and attends over the
     cached prefix (`vima_attention` with kv_batch_rows / mask_ld / q_pos0)."""
 
-    def __init__(self, *, B: int, Lmax: int, E: int, n_layer: int, device, split: bool, precision: str = ""):
+    def __init__(self, *, B: int, Lmax: int, E: int, n_layer: int, device, split: bool, precision: str = "", weights=None):
         self.B, self.Lmax, self.E, self.L = B, Lmax, E, 0
         self.precision = precision  # the operand format the K/V rows are stored in; forward_step refuses any other mode
+        self.weights = weights  # engine.WeightState of the decoder at open: the cached K/V were projected with these weights
         mk = lambda: torch.zeros((B * Lmax, 2 * E), dtype=torch.int16, device=device)
         self.kv_hi = [mk() for _ in range(n_layer)]
         self.kv_lo = [mk() if split else None for _ in range(n_layer)]
@@ -107,8 +108,9 @@ class SlotDecodeCache:
     reading the device.  A decoder-only model (HFGPT) opens it with Lp_cap = 0: its prompt and separator are the first columns of
     the self-attention cache (HFGPT.prefill), and there is no prompt_kv / prompt_mask."""
 
-    def __init__(self, *, S: int, Lmax: int, Lp_cap: int, E: int, n_layer: int, device, split: bool, precision: str):
+    def __init__(self, *, S: int, Lmax: int, Lp_cap: int, E: int, n_layer: int, device, split: bool, precision: str, weights=None):
         self.S, self.Lmax, self.Lp_cap, self.E, self.precision = S, Lmax, Lp_cap, E, precision
+        self.weights = weights  # engine.WeightState of the decoder at open; admit and step refuse once it has changed
         mk = lambda rows: torch.zeros((rows, 2 * E), dtype=torch.int16, device=device)
         self.kv_hi = [mk(S * Lmax) for _ in range(n_layer)]
         self.kv_lo = [mk(S * Lmax) if split else None for _ in range(n_layer)]
@@ -139,8 +141,10 @@ class SlotDecodeCache:
         self.check_precision(p)
 
     def check_precision(self, p) -> None:
+        """The mode and the weights the cache was opened with are still in force (its K/V rows were computed with them)."""
         if self.precision != p.name:
             raise ValueError(f"SlotDecodeCache was opened in precision mode {self.precision!r}; the current mode is {p.name!r}")
+        check_cache_weights(self)
 
     def advance_host(self, Q: int) -> None:
         """Host mirror of what vima_slot_step_end does on the device."""
@@ -168,6 +172,15 @@ def check_cache_append(cache: "DecodeCache", B: int, L: int, E: int, p) -> None:
         raise ValueError(f"DecodeCache(B={cache.B}, Lmax={cache.Lmax}) cannot take {L} more tokens at length {cache.L}")
     if cache.precision and cache.precision != p.name:
         raise ValueError(f"DecodeCache was opened in precision mode {cache.precision!r}; the current mode is {p.name!r}")
+    check_cache_weights(cache)
+
+
+def check_cache_weights(cache) -> None:
+    """A cache's K/V rows were projected with the weights in force when it was opened: refuse to mix them with new ones."""
+    why = None if cache.weights is None else cache.weights.changed()
+    if why is not None:
+        raise ValueError(f"{type(cache).__name__}: {why} since the cache was opened; its K/V rows belong to the old weights. "
+                         "Open a new cache.")
 
 
 def run_block(ctx, p, W, blk: "Block", x32, x16, c16, *, B, L, E, H, omask, chain_ln=None, want16=False, out_f32=None, cache=None,
@@ -329,7 +342,7 @@ class XAttnGPT(nn.Module):
             if isinstance(m, (nn.Linear, nn.Embedding)):
                 nn.init.normal_(m.weight, std=0.02)
         self._input_checked = False
-        self._wc = eng.WeightCache()
+        self._wc = eng.WeightCache(self)
         self._pos_guard = PosIdGuard()
 
     def check_errors(self):
@@ -555,7 +568,7 @@ class HFGPT(nn.Module):
         for m in self.modules():
             if isinstance(m, (nn.Linear, nn.Embedding)):
                 nn.init.normal_(m.weight, std=0.02)
-        self._wc = eng.WeightCache()
+        self._wc = eng.WeightCache(self)
         # checkpoints written with transformers 4.x carry `lm.h.N.attn.bias`; accept and ignore it
         self._register_load_state_dict_pre_hook(self._drop_causal_buffers)
 
@@ -570,6 +583,7 @@ class HFGPT(nn.Module):
         With `cache` (DecodeCache or SlotDecodeCache, opened by `prefill`) x, custom_mask and absolute position_ids describe only the
         tokens appended this step and only their rows are returned: a DecodeCache takes their mask columns and advances `L`; for a
         SlotDecodeCache x is one step block per slot as vima_slot_step_begin lays it out (it has written the mask columns)."""
+        eng.uses(self)  # fp32 parameters read by the kernels directly
         ctx = eng.ctx_for(x)
         p = eng.prec()
         if batch_first:
@@ -605,6 +619,7 @@ class HFGPT(nn.Module):
         mask columns [0, L) and the state are set: a SlotDecodeCache's by vima_slot_admit_prefix (len = L, n_valid = valid tokens,
         no action, active), a DecodeCache's (slots = all its rows, in order) by copying the mask and setting L and n_valid.  The
         caller has validated shapes, slots, capacity and the precision mode."""
+        eng.uses(self)  # fp32 parameters read by the kernels directly
         ctx = eng.ctx_for(x)
         p = eng.prec()
         L, n, E = x.shape

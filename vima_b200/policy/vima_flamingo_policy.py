@@ -58,12 +58,13 @@ class VIMAFlamingoPolicy(VIMAGatoPolicy):
         self._n_discrete_y_bins = 100
         self._n_discrete_z_bins = 50
         self._n_discrete_rot_bins = 50
-        self._wc = eng.WeightCache()
+        self._wc = eng.WeightCache(self)
         self._bins = {}
 
     def forward(self, obs_token: torch.Tensor, action_token: Optional[torch.Tensor], prompt_token: torch.Tensor, prompt_token_mask: torch.Tensor):
         """obs_token (T,B,4,E), action_token (T-1,B,E)|None, prompt_token (Lp,B,E), prompt_token_mask (B,Lp) -> (T,B,E)
         (vima_flamingo_policy.py:129-163)."""
+        eng.uses(self)  # fp32 parameters read by the kernels directly
         ctx = eng.ctx_for(obs_token)
         T, B, Q, E = obs_token.shape
         assert Q == self._obj_xf_num_queries

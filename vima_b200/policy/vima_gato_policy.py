@@ -56,7 +56,7 @@ class VIMAGatoPolicy(nn.Module):
         self._n_discrete_y_bins = 100
         self._n_discrete_z_bins = 50
         self._n_discrete_rot_bins = 50
-        self._wc = eng.WeightCache()
+        self._wc = eng.WeightCache(self)
         self._bins = {}
 
     @property
@@ -67,6 +67,7 @@ class VIMAGatoPolicy(nn.Module):
     def forward(self, obs_token: torch.Tensor, action_token: Optional[torch.Tensor], prompt_token: torch.Tensor, prompt_token_mask: torch.Tensor):
         """obs_token (T,B,Q,E), action_token (T-1,B,E)|None, prompt_token (Lp,B,E), prompt_token_mask (B,Lp) -> (T,B,E)
         (vima_gato_policy.py:120-191)."""
+        eng.uses(self)  # fp32 parameters read by the kernels directly
         ctx = eng.ctx_for(obs_token)
         T, B, Q, E = obs_token.shape
         assert Q == self._obj_xf_num_queries
@@ -112,6 +113,10 @@ class VIMAGatoPolicy(nn.Module):
         if Lp + 1 >= Lmax:
             raise ValueError(f"a prompt of {Lp} tokens + separator leaves no room in max_tokens={Lmax}")
 
+    def _decode_weights(self) -> "eng.WeightState":
+        """What a decode cache's rows are computed from: the decoder and the separator token (the step's tokens are the caller's)."""
+        return eng.WeightState([self.transformer], slots=[(self, "prompt_sep_token")])
+
     def _check_obs(self, Q: int) -> None:
         if Q != self._obj_xf_num_queries:
             raise ValueError(f"an observation is {self._obj_xf_num_queries} tokens, got {Q}")
@@ -129,7 +134,7 @@ class VIMAGatoPolicy(nn.Module):
         self._check_prompt(prompt_token, prompt_token_mask, B, Lmax)
         p = eng.prec()
         cache = vnn.DecodeCache(B=B, Lmax=Lmax, E=E, n_layer=self.transformer.n_layer, device=prompt_token.device, split=p.split,
-                                precision=p.name)
+                                precision=p.name, weights=self._decode_weights())
         cache.prefix = Lp + 1  # columns before the first step
         self.transformer.prefill(cache, list(range(B)), *self._prompt_prefix(ctx, prompt_token, prompt_token_mask))
         return cache
@@ -174,7 +179,7 @@ class VIMAGatoPolicy(nn.Module):
             raise ValueError("n_slots must be >= 1")
         p = eng.prec()
         return vnn.SlotDecodeCache(S=int(n_slots), Lmax=Lmax, Lp_cap=0, E=self.embed_dim, n_layer=self.transformer.n_layer, device=w.device,
-                                   split=p.split, precision=p.name)
+                                   split=p.split, precision=p.name, weights=self._decode_weights())
 
     def admit(self, cache, slots, prompt_token: torch.Tensor, prompt_token_mask: torch.Tensor) -> None:
         """Start a new episode in each of `slots` (replacing whatever they held): prompt_token (Lp,n,E), prompt_token_mask (n,Lp).
@@ -190,6 +195,7 @@ class VIMAGatoPolicy(nn.Module):
         self.transformer.prefill(cache, s, *self._prompt_prefix(ctx, prompt_token, prompt_token_mask))
 
     release = VIMAPolicy.release
+    refresh_weights = VIMAPolicy.refresh_weights
 
     def step_slots(self, cache, obs_token: torch.Tensor, action_token: Optional[torch.Tensor]) -> torch.Tensor:
         """One environment step of every slot: obs_token (1,S,Q,E), action_token (1,S,E) (each slot's previous action; ignored for
@@ -233,6 +239,7 @@ class VIMAGatoPolicy(nn.Module):
 
     def forward_prompt_assembly(self, prompts):
         """(token_types, word_batch, image_batch{"rgb": {view: (n_img,3,64,128)}}) -> (Lp,B,E), (B,Lp) bool (:193-251)."""
+        eng.uses(self)  # fp32 parameters read by the kernels directly
         raw_prompts_token_type, word_batch, image_batch = prompts
         ref = image_batch["rgb"][sorted(self._views)[0]]
         ctx = eng.ctx_for(ref)
@@ -285,6 +292,7 @@ class VIMAGatoPolicy(nn.Module):
 
     def forward_obs_token(self, obs):
         """obs {"rgb": {view: (T,B,3,64,128) u8}, "ee": (T,B)} -> (T,B,Q,E)  (:253-262)."""
+        eng.uses(self)  # fp32 parameters read by the kernels directly
         rgbs, ee = obs["rgb"], obs["ee"]
         lead = tuple(ee.shape[:2])
         ctx = eng.ctx_for(ee)

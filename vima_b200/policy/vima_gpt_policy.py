@@ -56,12 +56,13 @@ class VIMAGPTPolicy(VIMAGatoPolicy):
         self._n_discrete_y_bins = 100
         self._n_discrete_z_bins = 50
         self._n_discrete_rot_bins = 50
-        self._wc = eng.WeightCache()
+        self._wc = eng.WeightCache(self)
         self._bins = {}
 
     def forward(self, obs_token: torch.Tensor, action_token: Optional[torch.Tensor], prompt_token: torch.Tensor, prompt_token_mask: torch.Tensor):
         """obs_token (T,B,E), action_token (T-1,B,E)|None, prompt_token (Lp,B,E), prompt_token_mask (B,Lp) -> (T,B,E)
         (vima_gpt_policy.py:119-176): the Gato layout with one token per observation."""
+        eng.uses(self)  # fp32 parameters read by the kernels directly
         return VIMAGatoPolicy.forward(self, obs_token.unsqueeze(2), action_token, prompt_token, prompt_token_mask)
 
     # Cached and slot decode: VIMA-Gato's with one token per observation.  start_decode, open_slots, admit, release and
@@ -83,6 +84,7 @@ class VIMAGPTPolicy(VIMAGatoPolicy):
 
     def forward_obs_token(self, obs):
         """obs {"rgb": {view: (T,B,3,64,128) u8}, "ee": (T,B)} -> (T,B,E)  (vima_gpt_policy.py:240-251)."""
+        eng.uses(self)  # fp32 parameters read by the kernels directly
         rgbs, ee = obs["rgb"], obs["ee"]
         lead = tuple(ee.shape[:2])
         ctx = eng.ctx_for(ee)

@@ -54,14 +54,21 @@ class VIMAPolicy(nn.Module):
         self._n_discrete_y_bins = 100
         self._n_discrete_z_bins = 50
         self._n_discrete_rot_bins = 50
-        self._wc = eng.WeightCache()
+        self._wc = eng.WeightCache(self)
         self._bins = {}
+
+    def refresh_weights(self) -> None:
+        """Drop every packed weight (the next call repacks from the parameters as they are).  Call it after writing parameters
+        through `.data` (`param.data.copy_(t)`), which no version counter sees; every other update route is detected on its own
+        (INTEGRATION.md).  Graphs captured and decode caches opened before it refuse to run."""
+        eng.refresh_weights(self)
 
     # --------------------------------------------------------------------------------------------------
     def forward(self, obs_token: torch.Tensor, obs_mask: torch.Tensor, action_token: Optional[torch.Tensor], prompt_token: torch.Tensor,
                 prompt_token_mask: torch.Tensor):
         """obs_token (T,B,Q,E), obs_mask (T,B,Q) bool, action_token (T-1,B,E)|None, prompt_token (Lp,B,E),
         prompt_token_mask (B,Lp) bool -> predicted action tokens (T,B,E)   (vima_policy.py:116-159)."""
+        eng.uses(self)  # fp32 parameters read by the kernels directly
         ctx = eng.ctx_for(obs_token)
         T, B, Q, E = obs_token.shape
         La = 0 if action_token is None else action_token.shape[0]
@@ -97,7 +104,7 @@ class VIMAPolicy(nn.Module):
         if not 0 < Lmax <= self.xattn_gpt.n_positions:
             raise ValueError(f"max_tokens={Lmax} outside (0, n_positions={self.xattn_gpt.n_positions}]")
         cache = vnn.DecodeCache(B=B, Lmax=Lmax, E=E, n_layer=self.xattn_gpt.n_layer, device=prompt_token.device, split=eng.prec().split,
-                                precision=eng.prec().name)
+                                precision=eng.prec().name, weights=eng.WeightState([self.xattn_gpt]))
         pmask_u8 = eng.as_u8(prompt_token_mask)
         cache.prompt = (prompt_token, pmask_u8, self._prompt_positions(ctx, pmask_u8))
         return cache
@@ -156,7 +163,7 @@ class VIMAPolicy(nn.Module):
             raise ValueError("n_slots must be >= 1")
         p = eng.prec()
         return vnn.SlotDecodeCache(S=int(n_slots), Lmax=Lmax, Lp_cap=int(max_prompt_tokens), E=self.embed_dim, n_layer=self.xattn_gpt.n_layer,
-                                   device=dev, split=p.split, precision=p.name)
+                                   device=dev, split=p.split, precision=p.name, weights=eng.WeightState([self.xattn_gpt]))
 
     def admit(self, cache, slots, prompt_token: torch.Tensor, prompt_token_mask: torch.Tensor) -> None:
         """Start a new episode in each of `slots` (replacing whatever they held): prompt_token (Lp,n,E), prompt_token_mask (n,Lp),
@@ -224,6 +231,7 @@ class VIMAPolicy(nn.Module):
     # --------------------------------------------------------------------------------------------------
     def forward_prompt_assembly(self, prompts):
         """(token_types, word_batch, image_batch) -> prompt tokens (Lp,B,E), masks (B,Lp) bool  (vima_policy.py:161-240)."""
+        eng.uses(self)  # fp32 parameters read by the kernels directly
         raw_prompts_token_type, word_batch, image_batch = prompts
         ref = image_batch["cropped_img"][sorted(self._views)[0]]
         ctx = eng.ctx_for(ref)
@@ -285,6 +293,7 @@ class VIMAPolicy(nn.Module):
     # --------------------------------------------------------------------------------------------------
     def forward_obs_token(self, obs):
         """obs {"ee": (T,B) i64, "objects": {cropped_img,bbox,mask}x{front,top}} -> (T,B,Q,E), (T,B,Q) bool  (:242-259)."""
+        eng.uses(self)  # fp32 parameters read by the kernels directly
         objects, ee = obs["objects"], obs["ee"]
         lead = tuple(ee.shape[:2])
         ctx = eng.ctx_for(ee)
