@@ -319,6 +319,30 @@ int vima_action_postprocess(vima_ctx*, const int64_t* idx, int64_t n, int width,
 /* dists.py:20-28: per head log-softmax normalised logits and mode (first argmax of probs). head_off: DEVICE int[n_heads+1]. */
 int vima_head_select(vima_ctx*, const float* logits, int B, int n_heads, const int32_t* head_off_dev, float* logits_norm, int64_t* modes,
                      void* stream);
+/* Acting and scoring on the same heads (torch.distributions.Categorical(logits=...) per head, without torch's host RNG).  logits fp32
+ * [B, head_off[n_heads]], head_off DEVICE int[n_heads+1], as vima_head_select.  Per (row, head) the action is
+ *   - actions_in[row, head] when actions_in != NULL (scoring; actions_out is not written), else
+ *   - the mode, bit-identical to vima_head_select, when greedy != 0, else
+ *   - a draw from softmax(logits): u = (word 0 of Philox4x32-10 with key = seed (lo, hi words) and counter = (row, head, draw lo,
+ *     draw hi)) >> 8, times 2^-24; the first column with p > 0 whose running sum of exp(logit - max) exceeds u times the total
+ *     (lanes of a warp own consecutive 32-column chunks: a fixed summation order), or the last column with p > 0 if rounding
+ *     leaves none.  The draw index is the uint64 at counter_dev: every draw of the call reads it, and the call advances it by one
+ *     (a one-thread kernel after the sampling kernel; also when B == 0), so the host never passes it and graph replays draw fresh
+ *     numbers.
+ * Optional fp32 [B, n_heads] outputs: log_prob of the action (NaN for an action outside [0, dim)), entropy = -sum p log p over the
+ * p > 0 terms, both accumulated in fp64; logits_norm [B, head_off[n_heads]] as vima_head_select.  A head whose logits are all -inf
+ * gives action 0 and NaN log_prob and entropy.  No host synchronisation. */
+typedef struct {
+  uint32_t struct_size;    /* = sizeof(vima_head_sample_desc) of the caller's header */
+  const float* logits; int B; int n_heads; const int32_t* head_off_dev;
+  const int64_t* actions_in; /* [B, n_heads] or NULL (choose) */
+  int greedy;
+  uint64_t seed; uint64_t* counter_dev;
+  int64_t* actions_out;    /* [B, n_heads]; required unless actions_in is given */
+  float* log_prob; float* entropy; float* logits_norm;
+} vima_head_sample_desc;
+int vima_sizeof_head_sample_desc(void);
+int vima_head_sample(vima_ctx*, const vima_head_sample_desc* d, void* stream);
 
 #pragma GCC visibility pop
 #ifdef __cplusplus

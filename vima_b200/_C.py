@@ -87,6 +87,18 @@ class AttnDesc(C.Structure):
     ]
 
 
+class HeadSampleDesc(C.Structure):
+    _fields_ = [
+        ("struct_size", C.c_uint32),
+        ("logits", c_void_p), ("B", c_int), ("n_heads", c_int), ("head_off_dev", c_void_p),
+        ("actions_in", c_void_p),
+        ("greedy", c_int),
+        ("seed", C.c_uint64), ("counter_dev", c_void_p),
+        ("actions_out", c_void_p),
+        ("log_prob", c_void_p), ("entropy", c_void_p), ("logits_norm", c_void_p),
+    ]
+
+
 _lib: Optional[C.CDLL] = None
 
 EXPORTS = [
@@ -96,6 +108,7 @@ EXPORTS = [
     "vima_gather_prompt", "vima_patchify", "vima_vit_tokens", "vima_bbox_norm", "vima_fill_ee", "vima_max_u8",
     "vima_action_scale", "vima_action_postprocess", "vima_latent_attention", "vima_object_stats", "vima_crop_resize", "vima_head_select", "vima_gato_positions", "vima_pack_weight_f8", "vima_split_f8",
     "vima_slot_step_begin", "vima_slot_kv_append", "vima_slot_step_end", "vima_slot_kv_scatter", "vima_slot_admit_prefix",
+    "vima_head_sample", "vima_sizeof_head_sample_desc",
 ]
 
 
@@ -116,7 +129,8 @@ def load_library() -> C.CDLL:
             got = _lib.vima_abi_version()
             _lib = None
             raise RuntimeError(f"{LIB_PATH} speaks C-ABI v{got}, this package needs v{ABI_VERSION}: rebuild with `python -m vima_b200.build`")
-        for name, mirror in (("gemm_desc", GemmDesc), ("norm_desc", NormDesc), ("attn_desc", AttnDesc), ("f32_gemm_group", F32GemmGroup)):
+        for name, mirror in (("gemm_desc", GemmDesc), ("norm_desc", NormDesc), ("attn_desc", AttnDesc), ("f32_gemm_group", F32GemmGroup),
+                             ("head_sample_desc", HeadSampleDesc)):
             want = getattr(_lib, f"vima_sizeof_{name}")()
             if want != C.sizeof(mirror):  # the ctypes mirrors above and include/vima_b200.h have drifted apart
                 _lib = None
@@ -417,3 +431,15 @@ class Context:
     def head_select(self, logits, B, n_heads, head_off_i32, logits_norm, modes):
         self._ck(self.lib.vima_head_select(self.h, c_void_p(logits.data_ptr()), B, n_heads, c_void_p(head_off_i32.data_ptr()),
                                            c_void_p(_ptr(logits_norm)), c_void_p(modes.data_ptr()), c_void_p(self._s())), "head_select")
+
+    def head_sample(self, logits, B, n_heads, head_off_i32, *, actions_in=None, greedy=False, seed=0, counter=None, actions_out=None,
+                    log_prob=None, entropy=None, logits_norm=None):
+        """vima_head_sample: score actions_in (int64 [B, n_heads]), or choose the mode (greedy) or a Philox draw at the device draw
+        index `counter` (one uint64, advanced by the call) into actions_out."""
+        d = HeadSampleDesc()
+        d.struct_size = C.sizeof(HeadSampleDesc)
+        d.logits, d.B, d.n_heads, d.head_off_dev = logits.data_ptr(), int(B), int(n_heads), head_off_i32.data_ptr()
+        d.actions_in, d.greedy = _ptr(actions_in), int(bool(greedy))
+        d.seed, d.counter_dev = int(seed) & 0xFFFFFFFFFFFFFFFF, _ptr(counter)
+        d.actions_out, d.log_prob, d.entropy, d.logits_norm = _ptr(actions_out), _ptr(log_prob), _ptr(entropy), _ptr(logits_norm)
+        self._ck(self.lib.vima_head_sample(self.h, C.byref(d), c_void_p(self._s())), "head_sample")

@@ -4,9 +4,10 @@ import os
 import torch
 
 from .engine import get_precision, refresh_weights, set_precision
+from .nn.action import ActionSampler
 from .policy import VIMAFlamingoPolicy, VIMAGatoPolicy, VIMAGPTPolicy, VIMAPolicy
 
-__all__ = ["VIMAPolicy", "VIMAGatoPolicy", "VIMAGPTPolicy", "VIMAFlamingoPolicy", "create_policy_from_ckpt", "set_precision", "get_precision", "refresh_weights"]
+__all__ = ["VIMAPolicy", "VIMAGatoPolicy", "VIMAGPTPolicy", "VIMAFlamingoPolicy", "create_policy_from_ckpt", "set_precision", "get_precision", "refresh_weights", "ActionSampler"]
 
 
 def create_policy_from_ckpt(ckpt_path, device):

@@ -614,4 +614,28 @@ int vima_head_select(vima_ctx* c, const float* logits, int B, int n_heads, const
   LAUNCHED(c, launch_head_select(logits, B, n_heads, head_off_dev, logits_norm, (long long*)modes, (cudaStream_t)stream), "head_select");
 }
 
+int vima_head_sample(vima_ctx* c, const vima_head_sample_desc* desc, void* stream) {
+  CHECK_CTX(c);
+  vima_head_sample_desc d;
+  if (int rc = load_desc(c, desc, &d, sizeof(vima_head_sample_desc), "head_sample")) return rc;
+  const bool draw = !d.actions_in && !d.greedy;
+  if (d.B < 0 || d.n_heads <= 0 || (d.B > 0 && (!d.logits || !d.head_off_dev || (!d.actions_in && !d.actions_out))) ||
+      (draw && !d.counter_dev))
+    return fail(c, VIMA_E_INVALID, "head_sample: needs n_heads > 0, B >= 0, counter_dev when drawing, and for B > 0 logits, head_off "
+                                   "and actions_out unless actions_in is given");
+  HeadParams p = {};
+  p.logits = d.logits; p.B = d.B; p.n_heads = d.n_heads; p.head_off = d.head_off_dev;
+  p.mode = d.actions_in ? HEAD_SCORE : (d.greedy ? HEAD_SELECT : HEAD_SAMPLE);
+  p.actions_in = (const long long*)d.actions_in;
+  p.seed = d.seed;
+  p.counter = (const unsigned long long*)d.counter_dev;
+  p.actions_out = (long long*)d.actions_out;
+  p.log_prob = d.log_prob; p.entropy = d.entropy; p.logits_norm = d.logits_norm;
+  const cudaError_t e = launch_head_kernel(p, (cudaStream_t)stream);
+  if (e != cudaSuccess) return cuda_fail(c, e, "head_sample");
+  c->launches += head_kernel_launches(p);
+  return VIMA_OK;
+}
+int vima_sizeof_head_sample_desc(void) { return (int)sizeof(vima_head_sample_desc); }
+
 }  // extern "C"

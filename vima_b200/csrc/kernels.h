@@ -154,6 +154,22 @@ cudaError_t launch_action_post(const long long* idx, long long n, int width, con
                                int bound_stride, float* out, cudaStream_t s);
 cudaError_t launch_head_select(const float* logits, int B, int n_heads, const int* head_off, float* logits_norm, long long* modes,
                                cudaStream_t s);
+// The action-head kernel (misc.cu): per (row, head) the mode, a Philox draw from softmax(logits), or a given action; optionally the
+// log-probability of that action, the entropy and the log-softmax normalised logits.
+enum { HEAD_SELECT = 0, HEAD_SAMPLE = 1, HEAD_SCORE = 2 };
+struct HeadParams {
+  const float* logits; int B; int n_heads; const int* head_off;
+  int mode;
+  const long long* actions_in;            // HEAD_SCORE: [B, n_heads]
+  unsigned long long seed;                // HEAD_SAMPLE: Philox key
+  const unsigned long long* counter;      // HEAD_SAMPLE: draw index (device), advanced by launch_head_kernel
+  long long* actions_out;                 // HEAD_SELECT / HEAD_SAMPLE: [B, n_heads]
+  float* log_prob; float* entropy;        // [B, n_heads], optional
+  float* logits_norm;                     // [B, head_off[n_heads]], optional
+};
+cudaError_t launch_head_kernel(const HeadParams& p, cudaStream_t s);
+// kernels the launch enqueued (a sampling launch is followed by the counter's one-thread increment)
+inline int head_kernel_launches(const HeadParams& p) { return (p.B > 0) + (p.mode == HEAD_SAMPLE); }
 cudaError_t launch_gato_positions(const unsigned char* prompt_mask, int B, int Lp, int L, unsigned char* mask_out, long long* pos_out,
                                   cudaStream_t s);
 cudaError_t launch_max_u8(const unsigned char* x, long long n, int* out_max, cudaStream_t s);

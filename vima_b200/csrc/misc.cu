@@ -447,17 +447,81 @@ cudaError_t launch_action_post(const long long* idx, long long n, int width, con
   return cudaGetLastError();
 }
 
-// Per (episode, head): log-softmax normalised logits (Categorical(logits=...), dists.py:20-23) and the mode
-// = first argmax of the softmax probabilities (dists.py:25-28).  One warp per (b, head).
-__global__ void head_select_kernel(const float* __restrict__ logits, int B, int n_heads, const int* __restrict__ head_off,
-                                   float* __restrict__ logits_norm, long long* __restrict__ modes) {
+// Philox4x32-10 (Salmon et al., "Parallel random numbers: as easy as 1, 2, 3", SC'11), the Random123 round function and key schedule.
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
+#pragma unroll
+  for (int r = 0; r < 10; ++r) {
+    if (r) { k.x += 0x9E3779B9u; k.y += 0xBB67AE85u; }
+    const unsigned lo0 = 0xD2511F53u * c.x, hi0 = __umulhi(0xD2511F53u, c.x);
+    const unsigned lo1 = 0xCD9E8D57u * c.z, hi1 = __umulhi(0xCD9E8D57u, c.z);
+    c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
+  }
+  return c;
+}
+
+// Inverse-CDF draw over columns [o0, o1) of `row` with weights e_c = expf(row[c] - mx): lane l owns the 32 consecutive columns
+// [base + 32 l, base + 32 l + 32) of each 1024-column round; its running sum at column c is (carry + exclusive warp scan of the lane
+// sums) + the lane's own sequential sum up to c.  Returns the first column with e_c > 0 whose running sum exceeds u * (sum of all
+// e_c); when rounding leaves none (u * sum at or past the last partial sum), the last column with e_c > 0.  Offset from o0.
+__device__ __forceinline__ float head_lane_sum(const float* row, int c0, int o1, float mx) {
+  float s = 0.f;
+  for (int c = c0; c < min(c0 + 32, o1); ++c) s += expf(row[c] - mx);
+  return s;
+}
+__device__ __forceinline__ float warp_scan_incl(float v, int lane) {
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const float t = __shfl_up_sync(0xffffffffu, v, o);
+    if (lane >= o) v += t;
+  }
+  return v;
+}
+__device__ int head_draw(const float* row, int o0, int o1, float mx, float u, int lane) {
+  float total = 0.f;
+  for (int base = o0; base < o1; base += 1024)
+    total += __shfl_sync(0xffffffffu, warp_scan_incl(head_lane_sum(row, base + 32 * lane, o1, mx), lane), 31);
+  const float t = u * total;
+  float carry = 0.f;
+  int last_pos = -1;
+  for (int base = o0; base < o1; base += 1024) {
+    const int c0 = base + 32 * lane;
+    const float s = head_lane_sum(row, c0, o1, mx);
+    const float incl = warp_scan_incl(s, lane);
+    float excl = __shfl_up_sync(0xffffffffu, incl, 1);
+    if (lane == 0) excl = 0.f;
+    const float start = carry + excl;
+    int hit = -1;
+    float run = 0.f;
+    for (int c = c0; c < min(c0 + 32, o1); ++c) {
+      const float e = expf(row[c] - mx);
+      run += e;
+      if (e > 0.f) {
+        last_pos = c;
+        if (hit < 0 && start + run > t) hit = c;
+      }
+    }
+    const unsigned hits = __ballot_sync(0xffffffffu, hit >= 0);
+    if (hits) return __shfl_sync(0xffffffffu, hit, __ffs(hits) - 1) - o0;
+    carry += __shfl_sync(0xffffffffu, incl, 31);
+  }
+  // each lane's last_pos is its last positive column over every round, so the head's last one is the largest of them
+  last_pos = __reduce_max_sync(0xffffffffu, last_pos);
+  return last_pos >= 0 ? last_pos - o0 : 0;
+}
+
+// One warp per (row b, head).  Every mode computes the log-softmax normalised logits (Categorical(logits=...), dists.py:20-23) and
+// the mode = first argmax of the softmax probabilities (dists.py:25-28) exactly as vima_head_select always has; HEAD_SAMPLE then
+// draws the action from softmax(logits) with u = (Philox4x32-10(counter = (b, head, draw lo, draw hi), key = seed).x >> 8) * 2^-24,
+// HEAD_SCORE takes it from actions_in.  log_prob and entropy are accumulated in fp64 over d_c = logit_c - max.
+__global__ void head_kernel(const HeadParams p) {
   const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
-  if (w >= B * n_heads) return;
+  const int n_heads = p.n_heads;
+  if (w >= p.B * n_heads) return;
   const int b = w / n_heads, hd = w % n_heads;
-  const int o0 = head_off[hd], o1 = head_off[hd + 1];
-  const int total = head_off[n_heads];
-  const float* row = logits + (size_t)b * total;
+  const int o0 = p.head_off[hd], o1 = p.head_off[hd + 1];
+  const int total = p.head_off[n_heads];
+  const float* row = p.logits + (size_t)b * total;
   float mx = -INFINITY;
   for (int c = o0 + lane; c < o1; c += 32) mx = fmaxf(mx, row[c]);
   mx = warp_max(mx);
@@ -469,7 +533,7 @@ __global__ void head_select_kernel(const float* __restrict__ logits, int B, int 
   int best_i = 0x7fffffff;
   for (int c = o0 + lane; c < o1; c += 32) {
     const float ln = row[c] - lse;
-    if (logits_norm) logits_norm[(size_t)b * total + c] = ln;
+    if (p.logits_norm) p.logits_norm[(size_t)b * total + c] = ln;
     const float pr = expf(ln);
     if (pr > best) { best = pr; best_i = c - o0; }
   }
@@ -482,14 +546,69 @@ __global__ void head_select_kernel(const float* __restrict__ logits, int B, int 
   // a head whose logits are all -inf has NaN probabilities (and NaN normalised logits, as log_softmax gives): argmax over
   // them is index 0 in torch, and no lane found a probability to keep
   if (best_i == 0x7fffffff) best_i = 0;
-  if (lane == 0) modes[(size_t)b * n_heads + hd] = (long long)best_i;
+  const size_t oi = (size_t)b * n_heads + hd;
+  const bool dead = mx == -INFINITY;  // all -inf: index 0, NaN log-prob and entropy
+  long long act = best_i;
+  if (p.mode == HEAD_SAMPLE) {
+    const unsigned long long draw = *p.counter;
+    const uint4 r = philox4x32_10(make_uint4((unsigned)b, (unsigned)hd, (unsigned)draw, (unsigned)(draw >> 32)),
+                                  make_uint2((unsigned)p.seed, (unsigned)(p.seed >> 32)));
+    act = dead ? 0 : head_draw(row, o0, o1, mx, (float)(r.x >> 8) * 0x1p-24f, lane);
+  } else if (p.mode == HEAD_SCORE) {
+    act = p.actions_in[oi];
+  }
+  if (p.mode != HEAD_SCORE && lane == 0) p.actions_out[oi] = act;
+  if (!p.log_prob && !p.entropy) return;
+  double S = 0.0, T = 0.0;  // sum of exp(d_c), sum of exp(d_c) * d_c over the finite logits (p = 0 terms dropped)
+  for (int c = o0 + lane; c < o1; c += 32) {
+    const float x = row[c];
+    if (x != -INFINITY) {
+      const double d = (double)x - (double)mx;
+      const double e = exp(d);
+      S += e;
+      T += e * d;
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    S += __shfl_xor_sync(0xffffffffu, S, o);
+    T += __shfl_xor_sync(0xffffffffu, T, o);
+  }
+  if (lane != 0) return;
+  const double logS = log(S);
+  if (p.log_prob) {
+    const bool ok = !dead && act >= 0 && act < o1 - o0;
+    p.log_prob[oi] = ok ? (float)(((double)row[o0 + act] - (double)mx) - logS) : __int_as_float(0x7fc00000);
+  }
+  if (p.entropy) p.entropy[oi] = dead ? __int_as_float(0x7fc00000) : (float)(logS - T / S);
 }
+
+__global__ void counter_increment_kernel(unsigned long long* counter) { *counter += 1; }
+
+cudaError_t launch_head_kernel(const HeadParams& p, cudaStream_t s) {
+  if (p.B > 0) {
+    const int warps = p.B * p.n_heads;
+    head_kernel<<<(warps + 7) / 8, 256, 0, s>>>(p);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+  }
+  // every warp of the launch above reads the draw index; the increment runs once all of them have, so no replay or later launch
+  // ever reuses a draw.  A sampling call over no rows advances it too: the counter counts sampling calls.
+  if (p.mode == HEAD_SAMPLE) {
+    counter_increment_kernel<<<1, 1, 0, s>>>(const_cast<unsigned long long*>(p.counter));
+    return cudaGetLastError();
+  }
+  return cudaSuccess;
+}
+
 cudaError_t launch_head_select(const float* logits, int B, int n_heads, const int* head_off, float* logits_norm, long long* modes,
                                cudaStream_t s) {
-  if (B == 0) return cudaSuccess;
-  const int warps = B * n_heads;
-  head_select_kernel<<<(warps + 7) / 8, 256, 0, s>>>(logits, B, n_heads, head_off, logits_norm, modes);
-  return cudaGetLastError();
+  HeadParams p = {};
+  p.logits = logits; p.B = B; p.n_heads = n_heads; p.head_off = head_off;
+  p.mode = HEAD_SELECT;
+  p.actions_out = modes;
+  p.logits_norm = logits_norm;
+  return launch_head_kernel(p, s);
 }
 
 // Gato sequence layout (vima_gato_policy.py:150-182): mask = [prompt_mask | ones], position ids = arange over the

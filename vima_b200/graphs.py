@@ -25,6 +25,7 @@ import torch
 
 from . import _C
 from . import engine as eng
+from .nn.action import _GroupedMLPs
 
 
 def _map(fn, x, y=None):
@@ -97,46 +98,62 @@ class GraphedStep:
 
 
 class GraphedSlotStep:
-    """A policy's step_slots for one (S, Q), captured into a CUDA graph.  The slot state (len / n_valid / has_action / active) lives
-    on the device and the step's kernels read it, so admissions and releases between replays take effect.  Warm-up runs the step
-    (which advances the slots), so the state vectors and their host mirror are snapshotted first and restored afterwards; the K/V and
-    mask columns warm-up wrote lie at or past each slot's `len` and are never read before a step overwrites them.
+    """A policy's step_slots (or, with `act`, its act_slots) for one (S, Q), captured into a CUDA graph.  The slot state (len /
+    n_valid / has_action / active) lives on the device and the step's kernels read it, so admissions and releases between replays
+    take effect.  Warm-up runs the step (which advances the slots), so the state vectors, the fed-back action tokens, their host
+    mirror and the sampler's draw counter are snapshotted first and restored afterwards; the K/V and mask columns warm-up wrote lie
+    at or past each slot's `len` and are never read before a step overwrites them.
 
         g = policy.capture_step_slots(cache, obs, obs_mask, action)   # cache state unchanged
         out = g(obs, obs_mask, action)                                # = policy.step_slots(cache, obs, obs_mask, action)
+        g = policy.capture_act_slots(cache, obs, obs_mask, sampler=s) # cache state and s unchanged
+        actions, log_prob, entropy = g(obs, obs_mask)                 # = policy.act_slots(cache, obs, obs_mask, sampler=s)
 
     The step inputs are those of the policy's `_slot_step` after the cache: (obs_token, obs_mask, action_token) for VIMAPolicy,
-    (obs_token, action_token) for the baselines, whose obs tokens are all valid.  obs_token is (1,S,Q,E), or (1,S,E) with Q = 1."""
+    (obs_token, action_token) for the baselines, whose obs tokens are all valid; without the action token under `act`.  obs_token
+    is (1,S,Q,E), or (1,S,E) with Q = 1.  The closed loop's action heads run on buffers the graph owns."""
 
-    def __init__(self, policy, cache, obs_token: torch.Tensor, *inputs: torch.Tensor, warmup: int = 2):
+    def __init__(self, policy, cache, obs_token: torch.Tensor, *inputs: torch.Tensor, warmup: int = 2, act: bool = False, sampler=None):
         self.policy, self.cache = policy, cache
         self.S, self.E = obs_token.shape[1], obs_token.shape[-1]
         self.Q = obs_token.shape[2] if obs_token.dim() == 4 else 1
         cache.check_step(self.S, self.Q, self.E, eng.prec())
-        self.static_in = [obs_token.clone()] + [t.clone() for t in inputs[:-1]] + [inputs[-1].float().clone()]
+        if act:
+            self.static_in = [obs_token.clone()] + [t.clone() for t in inputs]
+            # the graph's own head buffers: allocated by the warm-up outside the graph's pool, their addresses are baked into the
+            # captured grouped GEMMs, so they must live as long as the graph
+            self.grouped = _GroupedMLPs()
+            step = lambda *a: policy._act_step(cache, *a, sampler=sampler, grouped=self.grouped)  # noqa: E731
+        else:
+            self.grouped = None
+            self.static_in = [obs_token.clone()] + [t.clone() for t in inputs[:-1]] + [inputs[-1].float().clone()]
+            step = lambda *a: policy._slot_step(cache, *a)  # noqa: E731
         dev = obs_token.device
         self.ctx = _C.Context.get(dev)
         saved = cache.state()
+        saved_draws = None if sampler is None else sampler.counter.clone()
         try:
             side = torch.cuda.Stream(device=dev)
             side.wait_stream(torch.cuda.current_stream(dev))
             with torch.cuda.stream(side):
                 for _ in range(max(warmup, 1)):  # packs weights, runs the first-call host checks, sets kernel attributes
-                    policy._slot_step(cache, *self.static_in)
+                    step(*self.static_in)
             torch.cuda.current_stream(dev).wait_stream(side)
             torch.cuda.synchronize(dev)
             self.graph = torch.cuda.CUDAGraph()
             n0 = self.ctx.launches
             with eng.record_weights() as weights, torch.cuda.graph(self.graph):
-                self.static_out = policy._slot_step(cache, *self.static_in)
+                self.static_out = step(*self.static_in)
             self.weights = weights()
             self.kernels_per_replay = self.ctx.launches - n0
         finally:
             cache.restore(saved)
+            if saved_draws is not None:
+                sampler.counter.copy_(saved_draws)
             torch.cuda.synchronize(dev)
         self.replays = 0
 
-    def __call__(self, obs_token: torch.Tensor, *inputs: torch.Tensor) -> torch.Tensor:
+    def __call__(self, obs_token: torch.Tensor, *inputs: torch.Tensor):
         if len(inputs) + 1 != len(self.static_in):
             raise ValueError(f"the graph was captured with {len(self.static_in)} step inputs, got {len(inputs) + 1}")
         check_weights(self.weights, precision=False)  # the cache refuses another precision mode (ValueError)

@@ -2,6 +2,7 @@
 from .action import (
     ActionDecoder,
     ActionEmbedding,
+    ActionSampler,
     Categorical,
     CategoricalNet,
     ContinuousActionEmbedding,

@@ -54,7 +54,11 @@ class _LazyCategorical:
 
 class MultiCategorical:
     """dists.py:12-28.  Built from raw logits (..., sum(action_dims)); normalisation + modes come from the
-    `head_select` kernel (dists.py:20-28: Categorical(logits) subtracts logsumexp; mode = argmax of probs)."""
+    `head_select` kernel (dists.py:20-28: Categorical(logits) subtracts logsumexp; mode = argmax of probs).
+
+    `sample`, `log_prob` and `entropy` run the action-head kernel on the raw logits, kept as `raw_logits`.  Each returns one value
+    per sub-head, (..., n_sub_heads); the sub-heads are independent, so the value of the joint action is the sum over the last
+    dimension."""
 
     def __init__(self, logits: torch.Tensor = None, action_dims: List[int] = None, *, _norm=None, _modes=None):
         self._action_dims = tuple(action_dims)
@@ -62,6 +66,7 @@ class MultiCategorical:
             assert logits.dim() >= 2, logits.shape
             assert logits.size(-1) == sum(self._action_dims), f"sum of action dims {self._action_dims} != {logits.size(-1)}"
             _norm, _modes = select_heads(logits, list(self._action_dims))
+        self.raw_logits = logits
         self._norm, self._modes = _norm, _modes
         offs, o = [], 0
         for n in self._action_dims:
@@ -72,8 +77,49 @@ class MultiCategorical:
     def mode(self):
         return self._modes
 
+    def sample(self, sampler: "ActionSampler") -> torch.Tensor:
+        """One draw per sub-head from softmax(logits) at temperature 1 (the semantics of Categorical(logits=...).sample()) from
+        `sampler`'s stream: int64 (..., n_sub_heads), laid out as `mode()`.  Advances the sampler by one draw."""
+        return sample_heads(self.raw_logits, self._action_dims, sampler=sampler)[0]
+
+    def log_prob(self, actions: torch.Tensor) -> torch.Tensor:
+        """Log-probability of the integer `actions` (..., n_sub_heads) under each sub-head: fp32 (..., n_sub_heads), NaN where an
+        index lies outside its sub-head."""
+        return sample_heads(self.raw_logits, self._action_dims, actions=actions, log_prob=True)[1]
+
+    def entropy(self) -> torch.Tensor:
+        """-sum p log p of each sub-head over its p > 0 terms: fp32 (..., n_sub_heads)."""
+        return sample_heads(self.raw_logits, self._action_dims, entropy=True)[2]
+
+
+class ActionSampler:
+    """The random stream of `MultiCategorical.sample` and of the policies' `act_slots`: a 64-bit seed and a draw counter in device
+    memory.  Draw n of a sampling launch uses Philox4x32-10 with key = seed and counter = (row, sub-head, n), and the launch itself
+    advances the counter on the device.  So CUDA-graph replays draw fresh numbers, and an eager run and a replayed run from the same
+    seed draw the same sequence.  One sampler serves one device and one stream at a time: launches on two streams would race for
+    the counter."""
+
+    def __init__(self, seed: int, device):
+        self.seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+        self.counter = torch.zeros(1, dtype=torch.int64, device=device)  # the uint64 draw index
+
+    @property
+    def draws(self) -> int:
+        """Sampling calls so far (one over no rows counts too).  Reads the device, so it synchronises: meant for tests."""
+        return int(self.counter.item())
+
 
 _head_off_cache: Dict[tuple, torch.Tensor] = {}
+
+
+def _head_off(dims, device) -> torch.Tensor:
+    key = (tuple(dims), str(device))
+    if key not in _head_off_cache:
+        off = [0]
+        for n in dims:
+            off.append(off[-1] + n)
+        _head_off_cache[key] = torch.tensor(off, dtype=torch.int32).to(device)
+    return _head_off_cache[key]
 
 
 def select_heads(logits: torch.Tensor, dims: List[int]):
@@ -82,16 +128,36 @@ def select_heads(logits: torch.Tensor, dims: List[int]):
     lead = logits.shape[:-1]
     total = sum(dims)
     x = logits.reshape(-1, total).float().contiguous()
-    key = (tuple(dims), str(x.device))
-    if key not in _head_off_cache:
-        off = [0]
-        for n in dims:
-            off.append(off[-1] + n)
-        _head_off_cache[key] = torch.tensor(off, dtype=torch.int32).to(x.device)
     norm = torch.empty_like(x)
     modes = torch.empty((x.shape[0], len(dims)), dtype=torch.int64, device=x.device)
-    ctx.head_select(x, x.shape[0], len(dims), _head_off_cache[key], norm, modes)
+    ctx.head_select(x, x.shape[0], len(dims), _head_off(dims, x.device), norm, modes)
     return norm.view(*lead, total), modes.view(*lead, len(dims))
+
+
+def sample_heads(logits: torch.Tensor, dims, *, sampler: Optional[ActionSampler] = None, actions: Optional[torch.Tensor] = None,
+                 log_prob: bool = False, entropy: bool = False):
+    """One launch of the action-head kernel on raw logits (..., sum(dims)) -> (actions, log_prob, entropy), each (..., len(dims))
+    or None.  The actions are `actions` when given (scored; returned as None), else a draw from `sampler`, else the modes."""
+    ctx = eng.ctx_for(logits)
+    lead = logits.shape[:-1]
+    n = len(dims)
+    x = logits.reshape(-1, sum(dims)).float().contiguous()
+    B, dev = x.shape[0], x.device
+    a_in = a_out = None
+    if actions is not None:
+        if tuple(actions.shape) != tuple(lead) + (n,):
+            raise ValueError(f"actions of shape {tuple(actions.shape)} for logits {tuple(logits.shape)} of {n} sub-heads")
+        a_in = actions.to(device=dev, dtype=torch.int64).reshape(B, n).contiguous()
+    else:
+        a_out = torch.empty((B, n), dtype=torch.int64, device=dev)
+    if sampler is not None and sampler.counter.device != dev:
+        raise ValueError(f"the sampler lives on {sampler.counter.device}, the logits on {dev}")
+    lp = torch.empty((B, n), dtype=torch.float32, device=dev) if log_prob else None
+    ent = torch.empty((B, n), dtype=torch.float32, device=dev) if entropy else None
+    ctx.head_sample(x, B, n, _head_off(dims, dev), actions_in=a_in, greedy=sampler is None,
+                    seed=0 if sampler is None else sampler.seed, counter=None if sampler is None else sampler.counter,
+                    actions_out=a_out, log_prob=lp, entropy=ent)
+    return tuple(None if t is None else t.view(*lead, n) for t in (a_out, lp, ent))
 
 
 class CategoricalHead(nn.Module):
@@ -208,10 +274,9 @@ class ActionDecoder(nn.Module):
     _grouped = _GroupedMLPs()
 
     @staticmethod
-    def run_heads(nets: List[nn.Module], x: torch.Tensor, grouped: Optional[_GroupedMLPs] = None):
-        """All heads of all nets in three grouped launches + one head_select launch; returns one dist per net."""
+    def head_logits(nets: List[nn.Module], x: torch.Tensor, grouped: Optional[_GroupedMLPs] = None):
+        """All heads of all nets in three grouped launches: (raw logits fp32 [rows, sum(dims)], dims, per net its (first, end) sub-head)."""
         grouped = grouped or ActionDecoder._grouped
-        lead = x.shape[:-1]
         x2 = x.reshape(-1, x.shape[-1]).float().contiguous()
         mlps, dims, spans = [], [], []
         for n in nets:
@@ -224,6 +289,16 @@ class ActionDecoder(nn.Module):
             offs.append(offs[-1] + n_)
         logits = torch.empty((x2.shape[0], offs[-1]), dtype=torch.float32, device=x.device)
         grouped.run(mlps, x2, logits, offs[:-1])
+        return logits, dims, spans
+
+    @staticmethod
+    def run_heads(nets: List[nn.Module], x: torch.Tensor, grouped: Optional[_GroupedMLPs] = None):
+        """All heads of all nets in three grouped launches + one head_select launch; returns one dist per net."""
+        lead = x.shape[:-1]
+        logits, dims, spans = ActionDecoder.head_logits(nets, x, grouped)
+        offs = [0]
+        for n_ in dims:
+            offs.append(offs[-1] + n_)
         norm, modes = select_heads(logits.view(*lead, offs[-1]), dims)
         out = []
         for net, (a, b) in zip(nets, spans):

@@ -104,6 +104,8 @@ class SlotDecodeCache:
     Self-attention K/V per layer: `kv_hi[i]` / `kv_lo[i]` [S*Lmax, 2E]; projected prompt K/V per layer: `prompt_kv[i]` (an Opnd
     [S*Lp_cap, 2E]) with `prompt_mask` [S, Lp_cap] (a shorter prompt's tail columns are masked).  Per-slot device state, int32 [S]:
     `len` (cache columns used), `n_valid` (next position id), `has_action`, `active`; `q_pos` is the step's scratch copy of `len`.
+    `action_token` fp32 [S, E] is the embedding of each slot's last action that `act_slots` feeds back to the next step (zero at open;
+    a slot's first step ignores it).
     The host mirrors len / has_action / active (it knows them from admissions and the step width), so capacity is checked without
     reading the device.  A decoder-only model (HFGPT) opens it with Lp_cap = 0: its prompt and separator are the first columns of
     the self-attention cache (HFGPT.prefill), and there is no prompt_kv / prompt_mask."""
@@ -119,6 +121,7 @@ class SlotDecodeCache:
         self.mask = torch.zeros((S, Lmax), dtype=torch.uint8, device=device)
         z = lambda: torch.zeros((S,), dtype=torch.int32, device=device)
         self.len, self.n_valid, self.has_action, self.active, self.q_pos = z(), z(), z(), z(), z()
+        self.action_token = torch.zeros((S, E), dtype=torch.float32, device=device)
         self.len_host = [0] * S
         self.has_action_host = [False] * S
         self.active_host = [False] * S
@@ -155,11 +158,11 @@ class SlotDecodeCache:
 
     def state(self) -> tuple:
         """Copies of the per-slot state (device vectors and host mirror)."""
-        return (tuple(t.clone() for t in (self.len, self.n_valid, self.has_action, self.active)),
+        return (tuple(t.clone() for t in (self.len, self.n_valid, self.has_action, self.active, self.action_token)),
                 (list(self.len_host), list(self.has_action_host), list(self.active_host)))
 
     def restore(self, st: tuple) -> None:
-        for dst, src in zip((self.len, self.n_valid, self.has_action, self.active), st[0]):
+        for dst, src in zip((self.len, self.n_valid, self.has_action, self.active, self.action_token), st[0]):
             dst.copy_(src)
         self.len_host, self.has_action_host, self.active_host = (list(x) for x in st[1])
 

@@ -237,6 +237,23 @@ class VIMAGatoPolicy(nn.Module):
         self._check_obs(1 if obs_token.dim() == 3 else obs_token.shape[2])
         return GraphedSlotStep(self, cache, obs_token, action_token, warmup=warmup)
 
+    # Closed loop: VIMAPolicy's with this class's _slot_step (VIMA-GPT and VIMA-Flamingo inherit both methods; VIMA-GPT's obs_token
+    # is (1,S,E)).
+    _act_slots = VIMAPolicy._act_slots
+    _act_step = VIMAPolicy._act_step
+
+    def act_slots(self, cache, obs_token: torch.Tensor, *, sampler=None):
+        """obs_token (1,S,Q,E) -> (actions, log_prob, entropy), as VIMAPolicy.act_slots with every obs token valid."""
+        self._check_obs(1 if obs_token.dim() == 3 else obs_token.shape[2])
+        return self._act_slots(cache, (obs_token,), sampler)
+
+    def capture_act_slots(self, cache, obs_token: torch.Tensor, *, sampler=None, warmup: int = 2):
+        """`act_slots` captured into one CUDA graph, as VIMAPolicy.capture_act_slots; call the result as g(obs_token)."""
+        from ..graphs import GraphedSlotStep
+
+        self._check_obs(1 if obs_token.dim() == 3 else obs_token.shape[2])
+        return GraphedSlotStep(self, cache, obs_token, warmup=warmup, act=True, sampler=sampler)
+
     def forward_prompt_assembly(self, prompts):
         """(token_types, word_batch, image_batch{"rgb": {view: (n_img,3,64,128)}}) -> (Lp,B,E), (B,Lp) bool (:193-251)."""
         eng.uses(self)  # fp32 parameters read by the kernels directly

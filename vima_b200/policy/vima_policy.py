@@ -228,6 +228,48 @@ class VIMAPolicy(nn.Module):
 
         return GraphedSlotStep(self, cache, obs_token, obs_mask, action_token, warmup=warmup)
 
+    # Closed loop (DESIGN.md 7 (f)5): step_slots, the action heads, the choice of action and its embedding, all on the device; the
+    # embedding goes to cache.action_token, the action input of the slot's next step.
+    def act_slots(self, cache, obs_token: torch.Tensor, obs_mask: torch.Tensor, *, sampler=None):
+        """One environment step of every slot that also acts: obs_token (1,S,Q,E), obs_mask (1,S,Q) -> (actions, log_prob, entropy),
+        dicts keyed like `forward_action_decoder(...)[k].mode()` with int64 / fp32 / fp32 tensors (1,S,n_k).  The action is each
+        head's mode when `sampler` is None, else a draw from `sampler` (vima_b200.ActionSampler; all heads of all keys are one
+        MultiCategorical in key order, one draw per call).  The step's action input is the embedding of each slot's previous action,
+        which the call itself left in cache.action_token."""
+        return self._act_slots(cache, (obs_token, obs_mask), sampler)
+
+    def _act_slots(self, cache, inputs, sampler):
+        """act_slots of all four policies: `inputs` are those of the policy's _slot_step before the action token."""
+        obs_token = inputs[0]
+        S, E = obs_token.shape[1], obs_token.shape[-1]
+        Q = obs_token.shape[2] if obs_token.dim() == 4 else 1
+        cache.check_step(S, Q, E, eng.prec())
+        if "_act_grouped" not in self.__dict__:  # head buffers of its own, apart from forward_action_decoder's (one shape resident)
+            self._act_grouped = vnn.action._GroupedMLPs()
+        out = self._act_step(cache, *inputs, sampler=sampler, grouped=self._act_grouped)
+        cache.advance_host(Q)
+        return out
+
+    def _act_step(self, cache, *inputs, sampler=None, grouped=None):
+        """The device side of act_slots (static shapes, no host synchronisation; captured by GraphedSlotStep)."""
+        S, E = cache.S, cache.E
+        x = self._slot_step(cache, *inputs, cache.action_token.view(1, S, E))
+        dec = self.action_decoder
+        eng.uses(dec)  # fp32 parameters read by the kernels directly
+        keys = list(dec._decoders.keys())
+        logits, dims, spans = vnn.ActionDecoder.head_logits([dec._decoders[k] for k in keys], x.view(S, E), grouped)
+        acts, lp, ent = vnn.action.sample_heads(logits, dims, sampler=sampler, log_prob=True, entropy=True)
+        out = tuple({k: t[:, a:b].view(1, S, b - a) for k, (a, b) in zip(keys, spans)} for t in (acts, lp, ent))
+        cache.action_token.copy_(self.forward_action_token(out[0]).view(S, E))
+        return out
+
+    def capture_act_slots(self, cache, obs_token: torch.Tensor, obs_mask: torch.Tensor, *, sampler=None, warmup: int = 2):
+        """`act_slots` for this (S, Q) captured into one CUDA graph (vima_b200.graphs.GraphedSlotStep); the cache's slot state, its
+        fed-back action tokens and the sampler's counter are left as they were.  Call the result as g(obs_token, obs_mask)."""
+        from ..graphs import GraphedSlotStep
+
+        return GraphedSlotStep(self, cache, obs_token, obs_mask, warmup=warmup, act=True, sampler=sampler)
+
     # --------------------------------------------------------------------------------------------------
     def forward_prompt_assembly(self, prompts):
         """(token_types, word_batch, image_batch) -> prompt tokens (Lp,B,E), masks (B,Lp) bool  (vima_policy.py:161-240)."""
