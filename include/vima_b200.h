@@ -218,9 +218,18 @@ typedef struct {
    * When set (causal only, no rel_bias), batch element b has query row i at key position q_pos[b] + i and Lk_b = q_pos[b] + Lq
    * keys; `Lk` then only bounds the capacity (q_pos[b] in [0, Lk - Lq]) and q_pos0 is ignored. */
   const int* q_pos;
+  /* ---- v5 end ---- */
+  /* v6 tail (an addition; the ABI version stays 5): paged k / v (slot decode).  DEVICE int32 [B, kv_page_ld] or NULL.  When set,
+   * key j of batch element b is row kv_pages[b*kv_page_ld + j/64]*64 + j%64 of k / v, a pool of kv_pool_pages 64-row pages
+   * (kv_batch_rows is ignored); an entry outside [0, kv_pool_pages) reads page 0.  Needs q_pos, no rel_bias,
+   * Lk <= kv_page_ld*64 and kv_pool_pages*64 < 2^31. */
+  const int32_t* kv_pages;
+  int kv_page_ld, kv_pool_pages;
 } vima_attn_desc;
 #define VIMA_ATTN_DESC_V4_SIZE offsetof(vima_attn_desc, q_pos)
-#define VIMA_ATTN_DESC_V5_SIZE sizeof(vima_attn_desc)
+#define VIMA_ATTN_DESC_V5_SIZE offsetof(vima_attn_desc, kv_pages)
+#define VIMA_ATTN_DESC_V6_SIZE sizeof(vima_attn_desc)
+#define VIMA_KV_PAGE_TOKENS 64 /* rows of one K/V page: the streaming attention kernel's key chunk */
 int vima_attention(vima_ctx*, const vima_attn_desc* d, void* stream);
 
 /* HF modeling_perceiver.py PerceiverSelfAttention (the resampler of vima/nn/obj_encoder/perceiver/perceiver.py:11-41), fp32:
@@ -255,6 +264,12 @@ int vima_slot_step_begin(vima_ctx*, const float* obs, const uint8_t* obs_mask, c
  * b*Lmax + q_pos[b] + r of kv [S*Lmax, ld_kv].  width, col0, ld_* multiples of 8 elements, 16-byte aligned bases. */
 int vima_slot_kv_append(vima_ctx*, const void* qkv_hi, const void* qkv_lo, int ld_qkv, int col0, int width, int S, int Lq, const int32_t* q_pos,
                         void* kv_hi, void* kv_lo, int ld_kv, int Lmax, void* stream);
+/* vima_slot_kv_append into a paged cache: cache column col of slot b is row pages[b*page_ld + col/64]*64 + col%64 of kv, a pool of
+ * pool_pages 64-row pages ([pool_pages*64, ld_kv]); pages: DEVICE int32 [S, page_ld].  Columns past page_ld*64 and writes to page 0
+ * (the zero page) or to an entry outside [1, pool_pages) are skipped. */
+int vima_slot_kv_append_paged(vima_ctx*, const void* qkv_hi, const void* qkv_lo, int ld_qkv, int col0, int width, int S, int Lq,
+                              const int32_t* q_pos, void* kv_hi, void* kv_lo, int ld_kv, const int32_t* pages, int page_ld, int pool_pages,
+                              void* stream);
 /* out[b] = x[b*(Q+1) + Q-1+has_action[b]] (fp32 rows of E, pitch ldx); then, for active slots, len += Q + has_action,
  * n_valid += sum(step_mask[b]), has_action = 1. */
 int vima_slot_step_end(vima_ctx*, const float* x, int ldx, int S, int Q, int E, const uint8_t* step_mask, int32_t* len, int32_t* n_valid,
@@ -264,6 +279,11 @@ int vima_slot_step_end(vima_ctx*, const float* x, int ldx, int S, int Q, int E, 
  * kv [S*Lmax, ld_kv]; slots: DEVICE int32 [n], distinct.  Lq <= Lmax; width, col0, ld_* multiples of 8 elements, 16-byte aligned. */
 int vima_slot_kv_scatter(vima_ctx*, const void* qkv_hi, const void* qkv_lo, int ld_qkv, int col0, int width, int n, int Lq, const int32_t* slots,
                          void* kv_hi, void* kv_lo, int ld_kv, int Lmax, void* stream);
+/* vima_slot_kv_scatter into a paged cache (page table and pool as vima_slot_kv_append_paged): prefill row (j, r) -> row
+ * pages[slots[j]*page_ld + r/64]*64 + r%64 of kv; Lq <= page_ld*64; writes to page 0 or outside the pool are skipped. */
+int vima_slot_kv_scatter_paged(vima_ctx*, const void* qkv_hi, const void* qkv_lo, int ld_qkv, int col0, int width, int n, int Lq,
+                               const int32_t* slots, void* kv_hi, void* kv_lo, int ld_kv, const int32_t* pages, int page_ld, int pool_pages,
+                               void* stream);
 /* For each admitted slot b = slots[j] (DEVICE int32 [n]): slot_mask[b, 0:Lp] = prompt_mask[j] (uint8 [n, Lp]), slot_mask[b, Lp] = 1;
  * len[b] = Lp+1, n_valid[b] = sum(prompt_mask[j] != 0) + 1, has_action[b] = 0, active[b] = 1.  Lp + 1 <= Lmax. */
 int vima_slot_admit_prefix(vima_ctx*, const int32_t* slots, int n, const uint8_t* prompt_mask, int Lp, int Lmax, uint8_t* slot_mask,

@@ -2,6 +2,8 @@
 
 Environment: AB_B episodes, AB_L history keys (causal self-attention, Lq = Lk = L), AB_LP cross-attention keys (prompt tokens, Lq = L),
 AB_LQ > 0 adds a decode case (AB_LQ new query rows over AB_L cached keys, queries last), AB_SPLIT formats, AB_MASKED.
+--paged: the decode case also runs as slot decode does (per-element q_pos), from contiguous K/V and from a pool of 64-row pages
+through a shuffled page table (seed 0), both printed (e.g. AB_LQ=33 AB_L=1024 python tools/attn_bench.py --paged).
 """
 import sys, os, math
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -39,8 +41,30 @@ for split in [int(x) for x in os.environ.get("AB_SPLIT", "0,1").split(",")]:
         for _ in range(5): ctx.attention(**kw)
         e1.record(); torch.cuda.synchronize()
         ms = e0.elapsed_time(e1) / 5
+        timed = [("", ms)]
+        if "--paged" in sys.argv and causal and Lq < Lk:
+            pl = -(-Lk // 64)
+            perm = torch.randperm(B * pl, generator=torch.Generator().manual_seed(0)).to(torch.int32) + 1
+            table = perm.view(B, pl).cuda()
+            rows = (table.long()[:, torch.arange(Lk) // 64] * 64 + torch.arange(Lk, device="cuda") % 64).view(-1)
+            pool = torch.zeros((B * pl + 1) * 64, 2 * E, dtype=torch.int16, device="cuda")
+            pool_lo = torch.zeros_like(pool) if split else None
+            pool[rows] = kv
+            if split:
+                pool_lo[rows] = kl
+            qp = torch.full((B,), Lk - Lq, dtype=torch.int32, device="cuda")
+            base = dict(kw, q_pos0=0, q_pos=qp, mask_ld=Lk)
+            for label, extra in (("q_pos contiguous", dict(kv_batch_rows=Lk)),
+                                 ("q_pos paged", dict(k=(pool, pool_lo, 2 * E, 0), v=(pool, pool_lo, 2 * E, E), kv_pages=table,
+                                                      kv_pool_pages=B * pl + 1))):
+                ctx.attention(**{**base, **extra}); torch.cuda.synchronize()
+                e0.record()
+                for _ in range(20): ctx.attention(**{**base, **extra})
+                e1.record(); torch.cuda.synchronize()
+                timed.append((" " + label, e0.elapsed_time(e1) / 20))
         # causal: the cached keys in full plus half the square of the new rows (half of Lq * Lk for Lq = Lk)
         pairs = Lq * (Lk - Lq) + Lq * Lq / 2 if causal else Lq * Lk
         fl = 4.0 * B * H * pairs * D
-        print(f"split={split} {name:12s} Lq={Lq:5d} Lk={Lk:5d} {ms:8.3f} ms   {fl/ms/1e9:7.1f} TF/s algorithmic (causal: visible half of the new rows' square)",
-              flush=True)
+        for label, ms in timed:
+            print(f"split={split} {name + label:12s} Lq={Lq:5d} Lk={Lk:5d} {ms:8.3f} ms   {fl/ms/1e9:7.1f} TF/s algorithmic (causal: visible half of the new rows' square)",
+                  flush=True)

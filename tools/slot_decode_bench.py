@@ -14,7 +14,9 @@ positions).  Every episode runs to its end in each of three runs, and each run r
   graph     the same schedule with the step replayed from one CUDA graph (capture time reported, not counted)
 
 Longer episodes need more decoder positions: `--policy gato --model gato_200M --n-positions 1024 --max-steps 45` gives each slot
-257 + 45 * 17 = 1022 columns.  The header line prints the K/V cache size (n_layer * S * Lmax * 2E * 4 bytes).
+257 + 45 * 17 = 1022 columns.  The header line prints the unpaged K/V size (n_layer * S * Lmax * 2E * 4 bytes), the slot runs'
+page pool (--kv-pool-tokens, default S * Lmax rounded up to 64-token pages per slot) and the schedule's peak and mean page count;
+each slot run reports the peak pages it used and torch.cuda.max_memory_allocated.
 
 Admission (the prompt key/value GEMMs of the new episodes) is included in the slot runs' totals and also reported on its own
 (CUDA events).  Weights are random (timing only).  Prints the GPU's name and power limit beside the numbers, one JSON line per run.
@@ -43,6 +45,27 @@ def gpu_info() -> str:
         return f"{torch.cuda.get_device_name()}, power limit not readable"
 
 
+def pages_per_tick(lengths, S: int, Q: int, prefix: int, page: int = 64) -> list:
+    """K/V pages the active slots own at each tick of the slot runs' schedule (a slot whose episode ended takes the next one before
+    the next tick): a slot at cache length len owns the pages of its columns [0, len + Q + 1) once the tick's step has reserved
+    them.  A new episode starts at len = prefix (prompt + separator of the decoder-only baselines, 0 otherwise); its first step adds
+    Q columns (the dummy row is overwritten), every later one Q + 1.  Host arithmetic only."""
+    queue = list(lengths)
+    remaining, length = [0] * S, [0] * S
+    out = []
+    while True:
+        for b in range(S):
+            if not remaining[b] and queue:
+                remaining[b], length[b] = queue.pop(0), prefix
+        active = [b for b in range(S) if remaining[b]]
+        if not active:
+            return out
+        out.append(sum(-(-(length[b] + Q + 1) // page) for b in active))
+        for b in active:
+            length[b] += Q + (length[b] != prefix)
+            remaining[b] -= 1
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--policy", default="vima", choices=["vima", "gato", "gpt", "flamingo"])
@@ -56,6 +79,9 @@ def main():
     ap.add_argument("--episodes", type=int, default=1024)
     ap.add_argument("--precision", default="f16f8")
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--kv-pool-tokens", type=int, default=None,
+                    help="K/V page pool of the slot runs, in tokens (default: slots * Lmax rounded up to pages; 'peak' sizes use the "
+                         "schedule's peak page count printed in the header)")
     ap.add_argument("--runs", default=None, help="default: lockstep,eager,graph (vima); reforward,lockstep,eager,graph (baselines)")
     a = ap.parse_args()
     if not torch.cuda.is_available():
@@ -100,18 +126,23 @@ def main():
     name = "" if vima else f"policy {a.policy}, "
     n_layer = pol.xattn_gpt.n_layer if hasattr(pol, "xattn_gpt") else pol.transformer.n_layer
     kv_bytes = n_layer * S * Lmax * 2 * E * 4  # per layer [S*Lmax, 2E] K|V as (hi, lo) 16-bit pairs
+    page_ld = -(-Lmax // 64)
+    pool_pages = S * page_ld if a.kv_pool_tokens is None else -(-a.kv_pool_tokens // 64)
+    pool_bytes = n_layer * (pool_pages + 1) * 64 * 2 * E * 4  # the slot runs' page pool, zero page included
+    sched = pages_per_tick(lengths, S, Q, prefix)
     print(f"# {info}; {name}model {a.model or '200M'}, {S} slots, Q={Q}, Lp={Lp}, {a.precision}; {a.episodes} episodes of 1..{a.max_steps} steps "
-          f"({total_steps} env-steps, seed {a.seed}); {Lmax} cache columns per slot, K/V cache {kv_bytes / 1e9:.2f} GB")
+          f"({total_steps} env-steps, seed {a.seed}); {Lmax} cache columns per slot, K/V cache {kv_bytes / 1e9:.2f} GB unpaged (S*Lmax), "
+          f"page pool {pool_pages} pages = {pool_bytes / 1e9:.2f} GB; the schedule's peak {max(sched)} pages, mean {sum(sched) / len(sched):.0f}")
 
     if vima:
         forward_step, step_slots = pol.forward_step, pol.step_slots
-        open_slots = lambda: pol.open_slots(S, max_tokens=Lmax, max_prompt_tokens=Lp)  # noqa: E731
+        open_slots = lambda: pol.open_slots(S, max_tokens=Lmax, max_prompt_tokens=Lp, kv_pool_tokens=a.kv_pool_tokens)  # noqa: E731
         capture = pol.capture_step_slots
         replay = lambda gs, o, m, x: gs(o, m, x)  # noqa: E731
     else:
         forward_step = lambda c, o, m, x: pol.forward_step(c, o, x)  # noqa: E731
         step_slots = lambda c, o, m, x: pol.step_slots(c, o, x)  # noqa: E731
-        open_slots = lambda: pol.open_slots(S, max_tokens=Lmax)  # noqa: E731
+        open_slots = lambda: pol.open_slots(S, max_tokens=Lmax, kv_pool_tokens=a.kv_pool_tokens)  # noqa: E731
         capture = lambda c, o, m, x: pol.capture_step_slots(c, o, x)  # noqa: E731
         replay = lambda gs, o, m, x: gs(o, x)  # noqa: E731
 
@@ -131,7 +162,7 @@ def main():
                 else:
                     pol.forward(obs_hist[:t + 1, :n], at, prompts[:, :n], pmask[:n])
                 ticks += 1
-        return ticks, 0.0
+        return ticks, 0.0, None
 
     def lockstep():
         ticks = 0
@@ -142,13 +173,13 @@ def main():
             for t in range(max(batch)):
                 forward_step(cache, obs_pool[t % 3][:, :n], msk[:, :n], None if t == 0 else act[:, :n])
                 ticks += 1
-        return ticks, 0.0
+        return ticks, 0.0, None
 
     def slotted(step, cache):
-        """Runs every episode through `cache`; returns (ticks, admission ms)."""
+        """Runs every episode through `cache`; returns (ticks, admission ms, peak K/V pages in use)."""
         queue = list(range(len(lengths)))
         remaining = [0] * S
-        adm_ms, ticks = [], 0
+        adm_ms, ticks, peak = [], 0, 0
         pending = list(range(S))  # free slots waiting for an episode
         while True:
             take = pending[:len(queue)]
@@ -166,6 +197,7 @@ def main():
             if not any(remaining):
                 break
             step(cache, obs_pool[ticks % 3], msk, act)
+            peak = max(peak, cache.kv_pages_total - cache.kv_pages_free)
             ticks += 1
             pending = []
             for b in range(S):
@@ -174,21 +206,25 @@ def main():
                     if remaining[b] == 0:
                         pending.append(b)
         torch.cuda.synchronize()
-        return ticks, sum(e0.elapsed_time(e1) for e0, e1 in adm_ms)
+        return ticks, sum(e0.elapsed_time(e1) for e0, e1 in adm_ms), peak
 
     results = []
     with torch.no_grad():
         # warm-up: modules, weight packing, kernel attributes
         c = open_slots()
-        pol.admit(c, list(range(S)), prompts, pmask)
+        n_w = min(S, c.kv_pages_total // -(-(prefix + 2 * Q + 2) // 64))  # slots the pool holds for two steps
+        pol.admit(c, list(range(n_w)), prompts[:, :n_w], pmask[:n_w])
         for _ in range(2):
             step_slots(c, obs_pool[0], msk, act)
-        cd = pol.start_decode(prompts, pmask, max_tokens=Lmax)
-        for t in range(2):
-            forward_step(cd, obs_pool[0], msk, None if t == 0 else act)
-        del c, cd
+        del c
+        if "lockstep" in runs:  # an unpaged [S*Lmax] cache
+            cd = pol.start_decode(prompts, pmask, max_tokens=Lmax)
+            for t in range(2):
+                forward_step(cd, obs_pool[0], msk, None if t == 0 else act)
+            del cd
         torch.cuda.synchronize()
         for name in runs:
+            cache = fn = None  # the previous run's cache goes before the next one is opened
             extra = {}
             if name == "reforward":
                 fn = reforward
@@ -199,18 +235,20 @@ def main():
                 fn = lambda: slotted(step_slots, cache)  # noqa: E731
             elif name == "graph":
                 cache = open_slots()
-                pol.admit(cache, list(range(S)), prompts, pmask)
+                n_cap = min(S, cache.kv_pages_total // -(-(prefix + Q + 1) // 64))  # a small pool cannot hold every slot's first step
+                pol.admit(cache, list(range(n_cap)), prompts[:, :n_cap], pmask[:n_cap])
                 t0 = time.perf_counter()
                 gs = capture(cache, obs_pool[0], msk, act)
                 torch.cuda.synchronize()
                 extra = {"capture_s": round(time.perf_counter() - t0, 3), "vima_kernels_per_replay": gs.kernels_per_replay}
-                pol.release(cache, list(range(S)))
+                pol.release(cache, list(range(n_cap)))
                 fn = lambda: slotted(lambda c, o, m, x: replay(gs, o, m, x), cache)  # noqa: E731
             else:
                 raise SystemExit(f"unknown run {name}")
             torch.cuda.synchronize()
             t0 = time.perf_counter()
-            ticks, adm = fn()
+            torch.cuda.reset_peak_memory_stats()
+            ticks, adm, peak = fn()
             torch.cuda.synchronize()
             dt = time.perf_counter() - t0
             r = {"run": name, "seconds": round(dt, 4), "ticks": ticks, "env_steps_per_s": round(total_steps / dt, 1),
@@ -222,6 +260,11 @@ def main():
             r["gpu"] = info
             r["cache_columns"] = Lmax
             r["kv_cache_bytes"] = kv_bytes
+            r["max_memory_allocated"] = torch.cuda.max_memory_allocated()
+            if peak is not None:
+                r["kv_pool_pages"] = pool_pages
+                r["kv_pool_bytes"] = pool_bytes
+                r["peak_pages_used"] = peak
             results.append(r)
             print(json.dumps(r), flush=True)
 

@@ -84,7 +84,12 @@ class AttnDesc(C.Structure):
         ("kv_batch_rows", c_int), ("mask_ld", c_int), ("q_pos0", c_int),
         # v5
         ("q_pos", c_void_p),
+        # v6 tail (ABI version 5): paged k / v
+        ("kv_pages", c_void_p), ("kv_page_ld", c_int), ("kv_pool_pages", c_int),
     ]
+
+
+KV_PAGE_TOKENS = 64  # include/vima_b200.h VIMA_KV_PAGE_TOKENS
 
 
 class HeadSampleDesc(C.Structure):
@@ -108,6 +113,7 @@ EXPORTS = [
     "vima_gather_prompt", "vima_patchify", "vima_vit_tokens", "vima_bbox_norm", "vima_fill_ee", "vima_max_u8",
     "vima_action_scale", "vima_action_postprocess", "vima_latent_attention", "vima_object_stats", "vima_crop_resize", "vima_head_select", "vima_gato_positions", "vima_pack_weight_f8", "vima_split_f8",
     "vima_slot_step_begin", "vima_slot_kv_append", "vima_slot_step_end", "vima_slot_kv_scatter", "vima_slot_admit_prefix",
+    "vima_slot_kv_append_paged", "vima_slot_kv_scatter_paged",
     "vima_head_sample", "vima_sizeof_head_sample_desc",
 ]
 
@@ -287,9 +293,11 @@ class Context:
         self._ck(self.lib.vima_norm(self.h, C.byref(d), c_void_p(self._s())), "norm")
 
     def attention(self, *, q, k, v, o, B, H, Lq, Lk, D, scale, causal=False, key_mask=None, rel_bias=None, dtype=DT_F16, o8=None,
-                  kv_batch_rows=0, mask_ld=0, q_pos0=0, q_pos=None):
+                  kv_batch_rows=0, mask_ld=0, q_pos0=0, q_pos=None, kv_pages=None, kv_pool_pages=0):
         """q, k, v, o: (hi, lo|None, ld, column offset) tuples over 16-bit operand buffers.  q_pos: int32 [B] on the device, the
-        causal position of each batch element's first query row (its key count is then q_pos[b] + Lq; Lk is the capacity)."""
+        causal position of each batch element's first query row (its key count is then q_pos[b] + Lq; Lk is the capacity).
+        kv_pages: int32 [B, page_ld] on the device, paged k / v: key j of element b is row kv_pages[b, j // 64] * 64 + j % 64 of k / v,
+        a pool of kv_pool_pages pages."""
         es = 2
 
         def at(t, off):
@@ -308,6 +316,9 @@ class Context:
         if q_pos is not None:
             assert q_pos.dtype == torch.int32 and q_pos.is_contiguous() and q_pos.numel() >= B
             d.q_pos = q_pos.data_ptr()
+        if kv_pages is not None:
+            assert kv_pages.dtype == torch.int32 and kv_pages.dim() == 2 and kv_pages.is_contiguous() and kv_pages.shape[0] >= B
+            d.kv_pages, d.kv_page_ld, d.kv_pool_pages = kv_pages.data_ptr(), kv_pages.shape[1], int(kv_pool_pages)
         if o8 is not None:  # (lo8, hi8) uint8 [rows, ld8]
             d.o_lo8, d.o_hi8, d.ldo8 = o8[0].data_ptr(), o8[1].data_ptr(), o8[0].stride(0)
         self._ck(self.lib.vima_attention(self.h, C.byref(d), c_void_p(self._s())), "attention")
@@ -345,6 +356,14 @@ class Context:
                                               int(S), int(Lq), c_void_p(q_pos.data_ptr()), c_void_p(kv_hi.data_ptr()), c_void_p(_ptr(kv_lo)),
                                               int(ld_kv), int(Lmax), c_void_p(self._s())), "slot_kv_append")
 
+    def slot_kv_append_paged(self, qkv_hi, qkv_lo, ld_qkv, col0, width, S, Lq, q_pos, kv_hi, kv_lo, ld_kv, pages, pool_pages):
+        """slot_kv_append into a paged cache: pages int32 [S, page_ld] (device) of page indices into kv [pool_pages*64, ld_kv]."""
+        assert pages.dtype == torch.int32 and pages.dim() == 2 and pages.is_contiguous()
+        self._ck(self.lib.vima_slot_kv_append_paged(self.h, c_void_p(qkv_hi.data_ptr()), c_void_p(_ptr(qkv_lo)), int(ld_qkv), int(col0),
+                                                    int(width), int(S), int(Lq), c_void_p(q_pos.data_ptr()), c_void_p(kv_hi.data_ptr()),
+                                                    c_void_p(_ptr(kv_lo)), int(ld_kv), c_void_p(pages.data_ptr()), pages.shape[1],
+                                                    int(pool_pages), c_void_p(self._s())), "slot_kv_append_paged")
+
     def slot_step_end(self, x, S, Q, E, step_mask, *, len_, n_valid, has_action, active, out):
         """x fp32 [S*(Q+1), >=E] -> out [S, E] (each slot's prediction row); advances the active slots' state."""
         self._ck(self.lib.vima_slot_step_end(self.h, c_void_p(x.data_ptr()), x.stride(0), int(S), int(Q), int(E), c_void_p(step_mask.data_ptr()),
@@ -357,6 +376,15 @@ class Context:
         self._ck(self.lib.vima_slot_kv_scatter(self.h, c_void_p(qkv_hi.data_ptr()), c_void_p(_ptr(qkv_lo)), int(ld_qkv), int(col0), int(width),
                                                int(n), int(Lq), c_void_p(slots.data_ptr()), c_void_p(kv_hi.data_ptr()), c_void_p(_ptr(kv_lo)),
                                                int(ld_kv), int(Lmax), c_void_p(self._s())), "slot_kv_scatter")
+
+    def slot_kv_scatter_paged(self, qkv_hi, qkv_lo, ld_qkv, col0, width, n, Lq, slots, kv_hi, kv_lo, ld_kv, pages, pool_pages):
+        """slot_kv_scatter into a paged cache: prefill row (j, r) -> row pages[slots[j], r // 64] * 64 + r % 64 of kv."""
+        assert slots.dtype == torch.int32 and slots.is_contiguous() and slots.numel() >= n
+        assert pages.dtype == torch.int32 and pages.dim() == 2 and pages.is_contiguous()
+        self._ck(self.lib.vima_slot_kv_scatter_paged(self.h, c_void_p(qkv_hi.data_ptr()), c_void_p(_ptr(qkv_lo)), int(ld_qkv), int(col0),
+                                                     int(width), int(n), int(Lq), c_void_p(slots.data_ptr()), c_void_p(kv_hi.data_ptr()),
+                                                     c_void_p(_ptr(kv_lo)), int(ld_kv), c_void_p(pages.data_ptr()), pages.shape[1],
+                                                     int(pool_pages), c_void_p(self._s())), "slot_kv_scatter_paged")
 
     def slot_admit_prefix(self, slots, prompt_mask_u8, Lmax, slot_mask, *, len_, n_valid, has_action, active):
         """slots int32 [n], prompt_mask uint8 [n, Lp] -> mask columns [0, Lp] of the admitted slots and their fresh state."""

@@ -11,6 +11,7 @@
 #include "kernels.h"
 
 using namespace vima;
+static_assert(VIMA_KV_PAGE_TOKENS == KV_PAGE_TOKENS, "page size of the C ABI and of the kernels");
 
 struct vima_ctx {
   int device;
@@ -385,6 +386,12 @@ int vima_attention(vima_ctx* c, const vima_attn_desc* d_in, void* stream) {
   p.o_lo8 = (unsigned char*)d->o_lo8; p.o_hi8 = (unsigned char*)d->o_hi8; p.ldo8 = d->ldo8;
   p.kv_batch_rows = d->kv_batch_rows; p.mask_ld = d->mask_ld; p.q_pos0 = d->q_pos0; p.q_batch_rows = 0;
   p.q_pos = d->q_pos;
+  p.kv_pages = d->kv_pages; p.kv_page_ld = d->kv_page_ld; p.kv_pool_pages = d->kv_pool_pages;
+  if (d->kv_pages && (!d->q_pos || d->rel_bias || d->kv_page_ld < 1 || d->kv_pool_pages < 1 || d->Lk > (long long)d->kv_page_ld * VIMA_KV_PAGE_TOKENS ||
+                      (long long)d->kv_pool_pages * VIMA_KV_PAGE_TOKENS > 0x7fffffffll))
+    return fail(c, VIMA_E_INVALID, "attention: paged k / v need q_pos, no relative bias, Lk <= kv_page_ld*%d (Lk %d, kv_page_ld %d) and "
+                "1 <= kv_pool_pages with kv_pool_pages*%d rows inside the 32-bit row range (kv_pool_pages %d)", VIMA_KV_PAGE_TOKENS, d->Lk,
+                d->kv_page_ld, VIMA_KV_PAGE_TOKENS, d->kv_pool_pages);
   if ((d->kv_batch_rows && d->kv_batch_rows < d->Lk) || (d->mask_ld && d->mask_ld < d->Lk) || d->q_pos0 < 0)
     return fail(c, VIMA_E_INVALID, "attention: kv_batch_rows / mask_ld must cover Lk, q_pos0 >= 0");
   if (d->q_pos && (!d->causal || d->rel_bias || d->Lq > d->Lk))
@@ -486,8 +493,26 @@ int vima_slot_kv_append(vima_ctx* c, const void* qkv_hi, const void* qkv_lo, int
       !al(qkv_hi) || !al(qkv_lo) || !al(kv_hi) || !al(kv_lo))
     return fail(c, VIMA_E_INVALID, "slot_kv_append: ld / col0 / width multiples of 8 inside the rows, 16-byte aligned bases, Lq <= Lmax");
   LAUNCHED(c, launch_slot_kv_append((const unsigned short*)qkv_hi, (const unsigned short*)qkv_lo, ld_qkv, col0, width, S, Lq, q_pos,
-                                    (unsigned short*)kv_hi, (unsigned short*)kv_lo, ld_kv, Lmax, (cudaStream_t)stream),
+                                    (unsigned short*)kv_hi, (unsigned short*)kv_lo, ld_kv, Lmax, nullptr, 0, (cudaStream_t)stream),
            "slot_kv_append");
+}
+
+int vima_slot_kv_append_paged(vima_ctx* c, const void* qkv_hi, const void* qkv_lo, int ld_qkv, int col0, int width, int S, int Lq,
+                              const int32_t* q_pos, void* kv_hi, void* kv_lo, int ld_kv, const int32_t* pages, int page_ld, int pool_pages,
+                              void* stream) {
+  CHECK_CTX(c);
+  if (!qkv_hi || !kv_hi || !q_pos || !pages || (qkv_lo == nullptr) != (kv_lo == nullptr))
+    return fail(c, VIMA_E_INVALID, "slot_kv_append_paged: null pointer");
+  auto al = [](const void* q) { return ((uintptr_t)q & 15) == 0; };
+  if ((ld_qkv & 7) || (col0 & 7) || (width & 7) || (ld_kv & 7) || width <= 0 || col0 < 0 || col0 + width > ld_qkv || width > ld_kv || Lq < 1 ||
+      page_ld < 1 || (long long)page_ld * VIMA_KV_PAGE_TOKENS > 0x7fffffffll || Lq > page_ld * VIMA_KV_PAGE_TOKENS || pool_pages < 1 ||
+      !al(qkv_hi) || !al(qkv_lo) || !al(kv_hi) || !al(kv_lo))
+    return fail(c, VIMA_E_INVALID, "slot_kv_append_paged: ld / col0 / width multiples of 8 inside the rows, 16-byte aligned bases, "
+                                   "page_ld >= 1, Lq <= page_ld*%d, pool_pages >= 1", VIMA_KV_PAGE_TOKENS);
+  LAUNCHED(c, launch_slot_kv_append((const unsigned short*)qkv_hi, (const unsigned short*)qkv_lo, ld_qkv, col0, width, S, Lq, q_pos,
+                                    (unsigned short*)kv_hi, (unsigned short*)kv_lo, ld_kv, page_ld * VIMA_KV_PAGE_TOKENS, pages, pool_pages,
+                                    (cudaStream_t)stream),
+           "slot_kv_append_paged");
 }
 
 int vima_slot_step_end(vima_ctx* c, const float* x, int ldx, int S, int Q, int E, const uint8_t* step_mask, int32_t* len, int32_t* n_valid,
@@ -508,8 +533,26 @@ int vima_slot_kv_scatter(vima_ctx* c, const void* qkv_hi, const void* qkv_lo, in
       Lq < 1 || Lq > Lmax || !al(qkv_hi) || !al(qkv_lo) || !al(kv_hi) || !al(kv_lo))
     return fail(c, VIMA_E_INVALID, "slot_kv_scatter: ld / col0 / width multiples of 8 inside the rows, 16-byte aligned bases, 1 <= Lq <= Lmax");
   LAUNCHED(c, launch_slot_kv_scatter((const unsigned short*)qkv_hi, (const unsigned short*)qkv_lo, ld_qkv, col0, width, n, Lq, slots,
-                                     (unsigned short*)kv_hi, (unsigned short*)kv_lo, ld_kv, Lmax, (cudaStream_t)stream),
+                                     (unsigned short*)kv_hi, (unsigned short*)kv_lo, ld_kv, Lmax, nullptr, 0, (cudaStream_t)stream),
            "slot_kv_scatter");
+}
+
+int vima_slot_kv_scatter_paged(vima_ctx* c, const void* qkv_hi, const void* qkv_lo, int ld_qkv, int col0, int width, int n, int Lq,
+                               const int32_t* slots, void* kv_hi, void* kv_lo, int ld_kv, const int32_t* pages, int page_ld, int pool_pages,
+                               void* stream) {
+  CHECK_CTX(c);
+  if (!qkv_hi || !kv_hi || !slots || !pages || (qkv_lo == nullptr) != (kv_lo == nullptr))
+    return fail(c, VIMA_E_INVALID, "slot_kv_scatter_paged: null pointer");
+  auto al = [](const void* q) { return ((uintptr_t)q & 15) == 0; };
+  if ((ld_qkv & 7) || (col0 & 7) || (width & 7) || (ld_kv & 7) || width <= 0 || col0 < 0 || col0 + width > ld_qkv || width > ld_kv || n < 0 ||
+      Lq < 1 || page_ld < 1 || (long long)page_ld * VIMA_KV_PAGE_TOKENS > 0x7fffffffll || Lq > page_ld * VIMA_KV_PAGE_TOKENS ||
+      pool_pages < 1 || !al(qkv_hi) || !al(qkv_lo) || !al(kv_hi) || !al(kv_lo))
+    return fail(c, VIMA_E_INVALID, "slot_kv_scatter_paged: ld / col0 / width multiples of 8 inside the rows, 16-byte aligned bases, "
+                                   "page_ld >= 1, 1 <= Lq <= page_ld*%d, pool_pages >= 1", VIMA_KV_PAGE_TOKENS);
+  LAUNCHED(c, launch_slot_kv_scatter((const unsigned short*)qkv_hi, (const unsigned short*)qkv_lo, ld_qkv, col0, width, n, Lq, slots,
+                                     (unsigned short*)kv_hi, (unsigned short*)kv_lo, ld_kv, page_ld * VIMA_KV_PAGE_TOKENS, pages, pool_pages,
+                                     (cudaStream_t)stream),
+           "slot_kv_scatter_paged");
 }
 
 int vima_slot_admit_prefix(vima_ctx* c, const int32_t* slots, int n, const uint8_t* prompt_mask, int Lp, int Lmax, uint8_t* slot_mask,

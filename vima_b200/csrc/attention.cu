@@ -61,7 +61,6 @@ __global__ void __launch_bounds__(256, (D == 32) ? 2 : 1) attention_kernel(const
   float* sbias = reinterpret_cast<float*>(qb_counter + 1);     // [2*Lk-1] (log2 domain) when rel_bias
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int kvb = p.kv_batch_rows ? p.kv_batch_rows : p.Lk;
   const int mld = p.mask_ld ? p.mask_ld : p.Lk;
   // ---- stage K (row-major) and V (transposed) of this (b, h) in shared memory ----
   constexpr int CH = D / 8;  // 16-byte chunks per row
@@ -69,8 +68,9 @@ __global__ void __launch_bounds__(256, (D == 32) ? 2 : 1) attention_kernel(const
     const int j = idx / CH, c = idx % CH;
     uint4 kh = make_uint4(0, 0, 0, 0), kl = kh, vh = kh, vl = kh;
     if (j < Lk) {
-      const size_t rk = ((size_t)b * kvb + j) * p.ldk + h * D + c * 8;
-      const size_t rv = ((size_t)b * kvb + j) * p.ldv + h * D + c * 8;
+      const size_t row = (size_t)attn_kv_row(p, b, j);
+      const size_t rk = row * p.ldk + h * D + c * 8;
+      const size_t rv = row * p.ldv + h * D + c * 8;
       kh = __ldg(reinterpret_cast<const uint4*>(p.k_hi + rk));
       vh = __ldg(reinterpret_cast<const uint4*>(p.v_hi + rv));
       if (SPLIT) {

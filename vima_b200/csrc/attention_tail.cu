@@ -44,7 +44,7 @@ __device__ __forceinline__ void ffma2(unsigned long long& acc, unsigned long lon
   acc = pack2(fmaf(y.x, z.x, x.x), fmaf(y.y, z.y, x.y));
 }
 
-template <int DT>
+template <int DT, bool PAGED>  // PAGED: k / v rows through the page table (attn_kv_row)
 __global__ void __launch_bounds__(TAIL_WARPS * 32) attention_tail_kernel(const AttnParams p, int row0, int nt, int lk_pad) {
   extern __shared__ __align__(16) float smt[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -52,7 +52,6 @@ __global__ void __launch_bounds__(TAIL_WARPS * 32) attention_tail_kernel(const A
   const long long unit = (long long)blockIdx.x * TAIL_WARPS + warp;
   if (unit >= (long long)p.B * p.H) return;  // whole warps leave; nothing below synchronises across warps
   const int b = (int)(unit / p.H), h = (int)(unit % p.H);
-  const int kvb = p.kv_batch_rows ? p.kv_batch_rows : p.Lk;
   const int mld = p.mask_ld ? p.mask_ld : p.Lk;
   const int qbr = p.q_batch_rows ? p.q_batch_rows : p.Lq;
   int qp0, Lk;  // this batch element's (per-batch with q_pos)
@@ -87,7 +86,7 @@ __global__ void __launch_bounds__(TAIL_WARPS * 32) attention_tail_kernel(const A
 #pragma unroll
     for (int c = 0; c < 4; ++c) { kh[c] = make_uint4(0u, 0u, 0u, 0u); kl[c] = kh[c]; }
     if (j < Lk) {
-      const size_t rk = ((size_t)b * kvb + j) * p.ldk + h * TAIL_D;
+      const size_t rk = (size_t)attn_kv_row<PAGED>(p, b, j) * p.ldk + h * TAIL_D;
       const uint4* ph = reinterpret_cast<const uint4*>(p.k_hi + rk);
 #pragma unroll
       for (int c = 0; c < 4; ++c) kh[c] = __ldg(ph + c);
@@ -173,7 +172,7 @@ __global__ void __launch_bounds__(TAIL_WARPS * 32) attention_tail_kernel(const A
       const int jj = j + 4 * u;
       vh[u] = make_uint2(0u, 0u); vl[u] = vh[u];
       if (jj < Lk) {
-        const size_t rv = ((size_t)b * kvb + jj) * p.ldv + h * TAIL_D + dg * 4;
+        const size_t rv = (size_t)attn_kv_row<PAGED>(p, b, jj) * p.ldv + h * TAIL_D + dg * 4;
         vh[u] = __ldg(reinterpret_cast<const uint2*>(p.v_hi + rv));
         if (p.v_lo) vl[u] = __ldg(reinterpret_cast<const uint2*>(p.v_lo + rv));
       }
@@ -231,6 +230,17 @@ __global__ void __launch_bounds__(TAIL_WARPS * 32) attention_tail_kernel(const A
   }
 }
 
+constexpr size_t TAIL_SMEM_MAX = (size_t)TAIL_WARPS * (TAIL_NT * TAIL_D + (size_t)ATTN_TAIL_MAX_LK * TAIL_NT) * sizeof(float);
+
+template <int DT, bool PAGED>
+cudaError_t launch_tail_t(const AttnParams& p, int row0, int nt, int lk_pad, unsigned grid, size_t smem, cudaStream_t stream) {
+  // the ceiling is the capacity's, so it is set once, whatever Lk the first call has
+  const cudaError_t e = raise_smem_ceiling<attention_tail_kernel<DT, PAGED>>((int)TAIL_SMEM_MAX);
+  if (e != cudaSuccess) return e;
+  attention_tail_kernel<DT, PAGED><<<grid, TAIL_WARPS * 32, smem, stream>>>(p, row0, nt, lk_pad);
+  return cudaGetLastError();
+}
+
 }  // namespace
 
 // rows [row0, row0 + nt) of every (batch, head) of p (nt <= ATTN_TAIL_MAX_ROWS); p.Lq / p.q_batch_rows give the row pitch
@@ -239,18 +249,12 @@ cudaError_t launch_attention_tail(const AttnParams& p, int row0, int nt, cudaStr
   if (nt > TAIL_NT || p.D != TAIL_D) return cudaErrorInvalidValue;
   const int lk_pad = (p.Lk + 31) & ~31;
   const size_t smem = (size_t)TAIL_WARPS * (TAIL_NT * TAIL_D + (size_t)lk_pad * TAIL_NT) * sizeof(float);
-  constexpr size_t smem_max = (size_t)TAIL_WARPS * (TAIL_NT * TAIL_D + (size_t)ATTN_TAIL_MAX_LK * TAIL_NT) * sizeof(float);
-  if (smem > smem_max) return cudaErrorInvalidValue;
-  const int fi = p.dtype == DT_BF16 ? 1 : 0;
-  // the ceiling is the capacity's, so it is set once, whatever Lk the first call has
-  const cudaError_t e = fi ? raise_smem_ceiling<attention_tail_kernel<DT_BF16>>((int)smem_max)
-                           : raise_smem_ceiling<attention_tail_kernel<DT_F16>>((int)smem_max);
-  if (e != cudaSuccess) return e;
+  if (smem > TAIL_SMEM_MAX) return cudaErrorInvalidValue;
   const long long units = (long long)p.B * p.H;
   const unsigned grid = (unsigned)((units + TAIL_WARPS - 1) / TAIL_WARPS);
-  if (fi) attention_tail_kernel<DT_BF16><<<grid, TAIL_WARPS * 32, smem, stream>>>(p, row0, nt, lk_pad);
-  else attention_tail_kernel<DT_F16><<<grid, TAIL_WARPS * 32, smem, stream>>>(p, row0, nt, lk_pad);
-  return cudaGetLastError();
+  const bool bf = p.dtype == DT_BF16;
+  if (p.kv_pages) return bf ? launch_tail_t<DT_BF16, true>(p, row0, nt, lk_pad, grid, smem, stream) : launch_tail_t<DT_F16, true>(p, row0, nt, lk_pad, grid, smem, stream);
+  return bf ? launch_tail_t<DT_BF16, false>(p, row0, nt, lk_pad, grid, smem, stream) : launch_tail_t<DT_F16, false>(p, row0, nt, lk_pad, grid, smem, stream);
 }
 
 }  // namespace vima

@@ -36,7 +36,20 @@ struct AttnParams {
   int q_pos0;                                  // causal: query row i sits at key position q_pos0 + i (incremental decode)
   int q_batch_rows;                            // rows between consecutive batch elements in q / o (>= Lq), 0 = Lq
   const int* q_pos;                            // causal, per batch element (device, or null): position q_pos[b], keys q_pos[b] + Lq
+  // paged k / v (slot decode): key j of batch element b is row kv_pages[b*kv_page_ld + j/64]*64 + j%64 of a pool of kv_pool_pages
+  // pages; null = the contiguous layout above
+  const int* kv_pages; int kv_page_ld; int kv_pool_pages;
 };
+constexpr int KV_PAGE_TOKENS = 64;  // = the streaming kernel's key chunk: one chunk is one page
+// k / v row of key j of batch element b.  A page entry outside [0, kv_pool_pages) reads as page 0 (the pool's zero page), so no
+// table contents can address memory outside the pool.  MAY_PAGE = false: the caller knows p is not paged (no run-time test).
+template <bool MAY_PAGE = true>
+__device__ __forceinline__ long long attn_kv_row(const AttnParams& p, int b, int j) {
+  if (!MAY_PAGE || p.kv_pages == nullptr) return (long long)b * (p.kv_batch_rows ? p.kv_batch_rows : p.Lk) + j;
+  int pg = __ldg(p.kv_pages + (size_t)b * p.kv_page_ld + j / KV_PAGE_TOKENS);
+  if ((unsigned)pg >= (unsigned)p.kv_pool_pages) pg = 0;
+  return (long long)pg * KV_PAGE_TOKENS + j % KV_PAGE_TOKENS;
+}
 // Attention scores are kept in the log2 domain: y = s * (scale*log2e) [+ bias*log2e]; the soft causal constant becomes
 // -1e4*log2e; the key-mask constant stays finfo.min (any value + finfo.min rounds to finfo.min, so "all masked keys are
 // equal" -- the reference's degenerate uniform row -- is preserved). softmax is invariant to the common factor.
@@ -86,6 +99,7 @@ cudaError_t launch_attention(const AttnParams& p, cudaStream_t stream);
 size_t attention_smem_bytes(const AttnParams& p);             // dynamic shared memory the mma.sync kernel needs for p
 int attention_max_lk(const AttnParams& p, size_t smem_limit);  // largest Lk (multiple of 64) that fits smem_limit at p's format
 // K/V-streaming wgmma kernel (attention_tc.cu, no length cap), one body with two entry points:
+long long attention_kv_rows(const AttnParams& p);      // rows of the k / v operands (the page pool's when paged)
 bool attention_tc_supported(const AttnParams& p);       // the decoders: head_dim 32, split operands, no bias
 bool attention_bias_tc_supported(const AttnParams& p);  // the T5 encoder: head_dim 64, relative bias, non-causal
 // runs p on the entry point its relative bias selects (p must pass one of the two predicates); encode_tiled_fn: cuTensorMapEncodeTiled
@@ -178,12 +192,16 @@ cudaError_t launch_max_u8(const unsigned char* x, long long n, int* out_max, cud
 cudaError_t launch_slot_step_begin(const float* obs, const unsigned char* obs_mask, const float* action, int S, int Q, int E, int Lmax,
                                    const int* len, const int* n_valid, const int* has_action, const int* active, float* tokens,
                                    unsigned char* step_mask, long long* pos, int* q_pos, unsigned char* slot_mask, cudaStream_t s);
+// The K/V writers take an optional page table (pages: int32 [rows, page_ld] of page indices into a pool of pool_pages pages, null =
+// the contiguous [S*Lmax] layout; Lmax is then page_ld*64).  Paged writes to page 0 (the zero page) or past the pool are skipped.
 cudaError_t launch_slot_kv_append(const unsigned short* qkv_hi, const unsigned short* qkv_lo, int ld_qkv, int col0, int width, int S, int Lq,
-                                  const int* q_pos, unsigned short* kv_hi, unsigned short* kv_lo, int ld_kv, int Lmax, cudaStream_t s);
+                                  const int* q_pos, unsigned short* kv_hi, unsigned short* kv_lo, int ld_kv, int Lmax, const int* pages,
+                                  int pool_pages, cudaStream_t s);
 cudaError_t launch_slot_step_end(const float* x, int ldx, int S, int Q, int E, const unsigned char* step_mask, int* len, int* n_valid,
                                  int* has_action, const int* active, float* out, cudaStream_t s);
 cudaError_t launch_slot_kv_scatter(const unsigned short* qkv_hi, const unsigned short* qkv_lo, int ld_qkv, int col0, int width, int n, int Lq,
-                                   const int* slots, unsigned short* kv_hi, unsigned short* kv_lo, int ld_kv, int Lmax, cudaStream_t s);
+                                   const int* slots, unsigned short* kv_hi, unsigned short* kv_lo, int ld_kv, int Lmax, const int* pages,
+                                   int pool_pages, cudaStream_t s);
 cudaError_t launch_slot_admit_prefix(const int* slots, int n, const unsigned char* prompt_mask, int Lp, int Lmax, unsigned char* slot_mask,
                                      int* len, int* n_valid, int* has_action, int* active, cudaStream_t s);
 

@@ -61,10 +61,18 @@ cudaError_t launch_slot_step_begin(const float* obs, const unsigned char* obs_ma
   return cudaGetLastError();
 }
 
-// Step rows (b, r) -> cache row b*Lmax + q_pos[b] + r, 8 16-bit values per thread and trip.
+// Destination row of cache column col (< Lmax) of slot b: b*Lmax + col, or with a page table (pages [*, Lmax/64]) row
+// page*64 + col%64 of the pool; -1 = skip (page 0, the zero page no slot owns, or an entry outside the pool).
+__device__ __forceinline__ long long slot_kv_row(int b, int col, int Lmax, const int* __restrict__ pages, int pool_pages) {
+  if (pages == nullptr) return (long long)b * Lmax + col;
+  const int pg = __ldg(pages + (size_t)b * (Lmax / KV_PAGE_TOKENS) + col / KV_PAGE_TOKENS);
+  return (pg <= 0 || pg >= pool_pages) ? -1 : (long long)pg * KV_PAGE_TOKENS + col % KV_PAGE_TOKENS;
+}
+
+// Step rows (b, r) -> cache column q_pos[b] + r of slot b, 8 16-bit values per thread and trip.
 __global__ void slot_kv_append_kernel(const uint4* __restrict__ qkv_hi, const uint4* __restrict__ qkv_lo, int ld_qkv8, int col8, int w8, int S,
                                       int Lq, const int* __restrict__ q_pos, uint4* __restrict__ kv_hi, uint4* __restrict__ kv_lo, int ld_kv8,
-                                      int Lmax) {
+                                      int Lmax, const int* __restrict__ pages, int pool_pages) {
   const long long total = (long long)S * Lq * w8;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const int c = (int)(i % w8);
@@ -72,21 +80,24 @@ __global__ void slot_kv_append_kernel(const uint4* __restrict__ qkv_hi, const ui
     const int r = (int)(br % Lq), b = (int)(br / Lq);
     const int col = q_pos[b] + r;
     if (col < 0 || col >= Lmax) continue;
+    const long long row = slot_kv_row(b, col, Lmax, pages, pool_pages);
+    if (row < 0) continue;
     const size_t src = (size_t)br * ld_qkv8 + col8 + c;
-    const size_t dst = ((size_t)b * Lmax + col) * ld_kv8 + c;
+    const size_t dst = (size_t)row * ld_kv8 + c;
     kv_hi[dst] = __ldg(qkv_hi + src);
     if (kv_lo) kv_lo[dst] = __ldg(qkv_lo + src);
   }
 }
 
 cudaError_t launch_slot_kv_append(const unsigned short* qkv_hi, const unsigned short* qkv_lo, int ld_qkv, int col0, int width, int S, int Lq,
-                                  const int* q_pos, unsigned short* kv_hi, unsigned short* kv_lo, int ld_kv, int Lmax, cudaStream_t s) {
+                                  const int* q_pos, unsigned short* kv_hi, unsigned short* kv_lo, int ld_kv, int Lmax, const int* pages,
+                                  int pool_pages, cudaStream_t s) {
   const long long total = (long long)S * Lq * (width / 8);
   if (total == 0) return cudaSuccess;
   const int blocks = (int)min((total + 255) / 256, (long long)132 * 16);
   slot_kv_append_kernel<<<blocks, 256, 0, s>>>(reinterpret_cast<const uint4*>(qkv_hi), reinterpret_cast<const uint4*>(qkv_lo), ld_qkv / 8,
                                                col0 / 8, width / 8, S, Lq, q_pos, reinterpret_cast<uint4*>(kv_hi),
-                                               reinterpret_cast<uint4*>(kv_lo), ld_kv / 8, Lmax);
+                                               reinterpret_cast<uint4*>(kv_lo), ld_kv / 8, Lmax, pages, pool_pages);
   return cudaGetLastError();
 }
 
@@ -120,31 +131,34 @@ cudaError_t launch_slot_step_end(const float* x, int ldx, int S, int Q, int E, c
 }
 
 // Admission of a decoder-only prompt (the prompt and its separator live in the self-attention cache, columns [0, Lq)).
-// Prefill rows (j, r) -> cache row slots[j]*Lmax + r, 8 16-bit values per thread and trip: each K/V element is read once and
+// Prefill rows (j, r) -> cache column r of slot slots[j], 8 16-bit values per thread and trip: each K/V element is read once and
 // written once.
 __global__ void slot_kv_scatter_kernel(const uint4* __restrict__ qkv_hi, const uint4* __restrict__ qkv_lo, int ld_qkv8, int col8, int w8, int n,
                                        int Lq, const int* __restrict__ slots, uint4* __restrict__ kv_hi, uint4* __restrict__ kv_lo, int ld_kv8,
-                                       int Lmax) {
+                                       int Lmax, const int* __restrict__ pages, int pool_pages) {
   const long long total = (long long)n * Lq * w8;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const int c = (int)(i % w8);
     const long long jr = i / w8;
     const int r = (int)(jr % Lq), j = (int)(jr / Lq);
+    const long long row = slot_kv_row(__ldg(slots + j), r, Lmax, pages, pool_pages);
+    if (row < 0) continue;
     const size_t src = (size_t)jr * ld_qkv8 + col8 + c;
-    const size_t dst = ((size_t)__ldg(slots + j) * Lmax + r) * ld_kv8 + c;
+    const size_t dst = (size_t)row * ld_kv8 + c;
     kv_hi[dst] = __ldg(qkv_hi + src);
     if (kv_lo) kv_lo[dst] = __ldg(qkv_lo + src);
   }
 }
 
 cudaError_t launch_slot_kv_scatter(const unsigned short* qkv_hi, const unsigned short* qkv_lo, int ld_qkv, int col0, int width, int n, int Lq,
-                                   const int* slots, unsigned short* kv_hi, unsigned short* kv_lo, int ld_kv, int Lmax, cudaStream_t s) {
+                                   const int* slots, unsigned short* kv_hi, unsigned short* kv_lo, int ld_kv, int Lmax, const int* pages,
+                                   int pool_pages, cudaStream_t s) {
   const long long total = (long long)n * Lq * (width / 8);
   if (total == 0) return cudaSuccess;
   const int blocks = (int)min((total + 255) / 256, (long long)132 * 16);
   slot_kv_scatter_kernel<<<blocks, 256, 0, s>>>(reinterpret_cast<const uint4*>(qkv_hi), reinterpret_cast<const uint4*>(qkv_lo), ld_qkv / 8,
                                                 col0 / 8, width / 8, n, Lq, slots, reinterpret_cast<uint4*>(kv_hi),
-                                                reinterpret_cast<uint4*>(kv_lo), ld_kv / 8, Lmax);
+                                                reinterpret_cast<uint4*>(kv_lo), ld_kv / 8, Lmax, pages, pool_pages);
   return cudaGetLastError();
 }
 

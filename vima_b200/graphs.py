@@ -100,9 +100,10 @@ class GraphedStep:
 class GraphedSlotStep:
     """A policy's step_slots (or, with `act`, its act_slots) for one (S, Q), captured into a CUDA graph.  The slot state (len /
     n_valid / has_action / active) lives on the device and the step's kernels read it, so admissions and releases between replays
-    take effect.  Warm-up runs the step (which advances the slots), so the state vectors, the fed-back action tokens, their host
-    mirror and the sampler's draw counter are snapshotted first and restored afterwards; the K/V and mask columns warm-up wrote lie
-    at or past each slot's `len` and are never read before a step overwrites them.
+    take effect, and so do K/V pages taken between replays (the graph reads the device page table).  Warm-up runs the step (which
+    advances the slots), so the state vectors, the fed-back action tokens, the page table, their host mirror, the page allocator
+    and the sampler's draw counter are snapshotted first and restored afterwards; the K/V and mask columns warm-up wrote lie at or
+    past each slot's `len` (in pages the slot owns, or skipped where it owns none) and are never read before a step overwrites them.
 
         g = policy.capture_step_slots(cache, obs, obs_mask, action)   # cache state unchanged
         out = g(obs, obs_mask, action)                                # = policy.step_slots(cache, obs, obs_mask, action)
@@ -160,6 +161,7 @@ class GraphedSlotStep:
         self.cache.check_step(obs_token.shape[1], obs_token.shape[2] if obs_token.dim() == 4 else 1, obs_token.shape[-1], eng.prec())
         if tuple(obs_token.shape) != tuple(self.static_in[0].shape):
             raise ValueError(f"the graph was captured for obs_token {tuple(self.static_in[0].shape)}, got {tuple(obs_token.shape)}")
+        self.cache.reserve_step(self.Q)  # the graph reads the device page table: pages taken here are the ones it writes and reads
         for dst, src in zip(self.static_in, (obs_token,) + inputs):
             if dst.data_ptr() != src.data_ptr():
                 dst.copy_(src, non_blocking=True)

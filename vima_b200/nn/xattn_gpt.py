@@ -98,24 +98,86 @@ class DecodeCache:
             self.kv_lo[i].view(B, self.Lmax, 2 * E)[:, L0:L0 + Ln].copy_(qkv16.lo.view(B, Ln, -1)[:, :, E:3 * E])
 
 
+class KVPagePool:
+    """Host allocator of a paged slot K/V cache (DESIGN.md 7 (f)1): pages 1 .. n_pages-1 of KV_PAGE_TOKENS cache columns each; page 0
+    is the zero page that no slot owns.  `owned[b]` lists the pages of slot b's columns [0, 64*len(owned[b])) in column order, so
+    row b of the page table is owned[b] followed by zeros.  `free` is the free list (taken from its end).  Pure Python: the cache
+    pushes the table entries that each call returns, as (flat index b*page_ld + k, page) pairs."""
+
+    def __init__(self, S: int, page_ld: int, n_pages: int):
+        if n_pages < 2:
+            raise ValueError(f"a page pool needs the zero page and at least one more, got {n_pages} pages")
+        self.S, self.page_ld, self.n_pages = S, page_ld, n_pages
+        self.free = list(range(n_pages - 1, 0, -1))
+        self.owned = [[] for _ in range(S)]
+
+    @staticmethod
+    def pages_for(cols: int) -> int:
+        return -(-cols // _C.KV_PAGE_TOKENS)
+
+    def needed(self, b: int, cols: int) -> int:
+        """New pages slot b needs so that it owns columns [0, cols)."""
+        return max(0, self.pages_for(cols) - len(self.owned[b]))
+
+    def reserve(self, b: int, cols: int) -> list:
+        """Give slot b pages up to column `cols` (the caller has checked `needed` against the free list)."""
+        own = self.owned[b]
+        upd = []
+        for _ in range(self.needed(b, cols)):
+            pg = self.free.pop()
+            upd.append((b * self.page_ld + len(own), pg))
+            own.append(pg)
+        return upd
+
+    def release(self, b: int) -> list:
+        """Return slot b's pages to the free list; its table row goes back to zeros."""
+        own = self.owned[b]
+        upd = [(b * self.page_ld + k, 0) for k in range(len(own))]
+        self.free.extend(reversed(own))
+        self.owned[b] = []
+        return upd
+
+    def state(self) -> tuple:
+        return list(self.free), [list(o) for o in self.owned]
+
+    def restore(self, st: tuple) -> None:
+        self.free, self.owned = list(st[0]), [list(o) for o in st[1]]
+
+
 class SlotDecodeCache:
     """K/V cache of `S` slots, each holding one episode at its own history length (DESIGN.md 4 and 7 (f)1).
 
-    Self-attention K/V per layer: `kv_hi[i]` / `kv_lo[i]` [S*Lmax, 2E]; projected prompt K/V per layer: `prompt_kv[i]` (an Opnd
-    [S*Lp_cap, 2E]) with `prompt_mask` [S, Lp_cap] (a shorter prompt's tail columns are masked).  Per-slot device state, int32 [S]:
-    `len` (cache columns used), `n_valid` (next position id), `has_action`, `active`; `q_pos` is the step's scratch copy of `len`.
-    `action_token` fp32 [S, E] is the embedding of each slot's last action that `act_slots` feeds back to the next step (zero at open;
-    a slot's first step ignores it).
-    The host mirrors len / has_action / active (it knows them from admissions and the step width), so capacity is checked without
-    reading the device.  A decoder-only model (HFGPT) opens it with Lp_cap = 0: its prompt and separator are the first columns of
-    the self-attention cache (HFGPT.prefill), and there is no prompt_kv / prompt_mask."""
+    Self-attention K/V per layer: `kv_hi[i]` / `kv_lo[i]`, a pool of `kv_pages_total + 1` pages of 64 rows [(P+1)*64, 2E] (page 0
+    is the zero page); `page_table` int32 [S, ceil(Lmax/64)] on the device maps column j of slot b to row page_table[b, j//64]*64 +
+    j%64 (0 = no page: reads see zeros, writes are skipped), and `pages` (KVPagePool) is its host mirror with the free list.  A slot
+    takes pages on the host before each step (check_step / reserve_step, the step's columns [0, len + Q + 1)) and returns them on
+    release or re-admission.  Projected prompt K/V per layer: `prompt_kv[i]` (an Opnd [S*Lp_cap, 2E]) with `prompt_mask` [S, Lp_cap]
+    (a shorter prompt's tail columns are masked).  Per-slot device state, int32 [S]: `len` (cache columns used), `n_valid` (next
+    position id), `has_action`, `active`; `q_pos` is the step's scratch copy of `len`.  `action_token` fp32 [S, E] is the embedding
+    of each slot's last action that `act_slots` feeds back to the next step (zero at open; a slot's first step ignores it).
+    The host mirrors len / has_action / active (it knows them from admissions and the step width), so capacity and pages are
+    checked and allocated without reading the device.  A decoder-only model (HFGPT) opens it with Lp_cap = 0: its prompt and
+    separator are the first columns of the self-attention cache (HFGPT.prefill), and there is no prompt_kv / prompt_mask.
 
-    def __init__(self, *, S: int, Lmax: int, Lp_cap: int, E: int, n_layer: int, device, split: bool, precision: str, weights=None):
+    kv_pool_tokens: cache columns the pool holds across all slots (rounded up to pages); None = S*ceil(Lmax/64) pages, so that
+    every slot can reach Lmax at once.  A smaller pool overcommits: a step or admission the free pages cannot cover raises
+    ValueError before any state is touched (`kv_pages_needed` tells a driver how many the next step takes)."""
+
+    def __init__(self, *, S: int, Lmax: int, Lp_cap: int, E: int, n_layer: int, device, split: bool, precision: str, weights=None,
+                 kv_pool_tokens: Optional[int] = None):
         self.S, self.Lmax, self.Lp_cap, self.E, self.precision = S, Lmax, Lp_cap, E, precision
         self.weights = weights  # engine.WeightState of the decoder at open; admit and step refuse once it has changed
+        page_ld = KVPagePool.pages_for(Lmax)
+        n_use = S * page_ld if kv_pool_tokens is None else KVPagePool.pages_for(int(kv_pool_tokens))
+        if not 1 <= n_use <= S * page_ld:
+            raise ValueError(f"kv_pool_tokens={kv_pool_tokens} must cover 1 .. {S * page_ld} pages of {_C.KV_PAGE_TOKENS} tokens "
+                             f"({S} slots of max_tokens={Lmax})")
+        self.pages = KVPagePool(S, page_ld, n_use + 1)
+        self.page_table = torch.zeros((S, page_ld), dtype=torch.int32, device=device)
         mk = lambda rows: torch.zeros((rows, 2 * E), dtype=torch.int16, device=device)
-        self.kv_hi = [mk(S * Lmax) for _ in range(n_layer)]
-        self.kv_lo = [mk(S * Lmax) if split else None for _ in range(n_layer)]
+        rows = self.pages.n_pages * _C.KV_PAGE_TOKENS
+        self.kv_hi = [mk(rows) for _ in range(n_layer)]
+        self.kv_lo = [mk(rows) if split else None for _ in range(n_layer)]
         self.prompt_kv = [eng.Opnd(S * Lp_cap, 2 * E, device, split, zero=True) for _ in range(n_layer)] if Lp_cap else None
         self.prompt_mask = torch.zeros((S, Lp_cap), dtype=torch.uint8, device=device) if Lp_cap else None
         self.mask = torch.zeros((S, Lmax), dtype=torch.uint8, device=device)
@@ -125,6 +187,19 @@ class SlotDecodeCache:
         self.len_host = [0] * S
         self.has_action_host = [False] * S
         self.active_host = [False] * S
+
+    @property
+    def kv_pages_total(self) -> int:
+        """Pages the slots can own (the pool without its zero page)."""
+        return self.pages.n_pages - 1
+
+    @property
+    def kv_pages_free(self) -> int:
+        return len(self.pages.free)
+
+    def kv_pages_needed(self, Q: int) -> int:
+        """New pages the next step of Q obs tokens takes: every active slot must own its columns [0, len + Q + 1)."""
+        return sum(self.pages.needed(b, self.len_host[b] + Q + 1) for b in range(self.S) if self.active_host[b])
 
     def slot_index(self, slots) -> list:
         s = [int(x) for x in (slots.tolist() if isinstance(slots, torch.Tensor) else slots)]
@@ -141,7 +216,53 @@ class SlotDecodeCache:
         full = [b for b in range(self.S) if self.active_host[b] and self.len_host[b] + Q + 1 > self.Lmax]
         if full:
             raise ValueError(f"slots {full} cannot take {Q + 1} more tokens (Lmax={self.Lmax}, lengths {[self.len_host[b] for b in full]})")
+        need = self.kv_pages_needed(Q)
+        if need > self.kv_pages_free:
+            raise ValueError(f"the step needs {need} more K/V pages, {self.kv_pages_free} of {self.kv_pages_total} are free: release "
+                             "slots or open the cache with a larger kv_pool_tokens")
         self.check_precision(p)
+
+    def reserve_step(self, Q: int) -> None:
+        """Take the pages the next step needs (after check_step, so it cannot fail); asynchronous, no host synchronisation."""
+        upd = []
+        for b in range(self.S):
+            if self.active_host[b]:
+                upd += self.pages.reserve(b, self.len_host[b] + Q + 1)
+        self._push_pages(upd)
+
+    def check_prefix(self, slots: list, cols: int) -> None:
+        """Refuses (before any state is touched) an admission of `slots` whose first `cols` columns the pool cannot cover, counting
+        the pages the slots give back."""
+        need = len(slots) * self.pages.pages_for(cols)
+        have = self.kv_pages_free + sum(len(self.pages.owned[b]) for b in slots)
+        if need > have:
+            raise ValueError(f"admitting {len(slots)} prefixes of {cols} tokens needs {need} K/V pages, {have} are free: release "
+                             "slots or open the cache with a larger kv_pool_tokens")
+
+    def free_slots(self, slots: list, prefix_cols: int = 0) -> None:
+        """Return the pages of `slots` (released or re-admitted) and give each `prefix_cols` columns of new ones (checked by
+        check_prefix).  Asynchronous, no host synchronisation."""
+        upd = []
+        for b in slots:
+            upd += self.pages.release(b)
+        for b in slots:
+            upd += self.pages.reserve(b, prefix_cols)
+        self._push_pages(upd)
+
+    def _push_pages(self, upd: list) -> None:
+        """Page-table entries (flat index, page) -> the device table: one copy from pinned host memory and one scatter, both queued
+        on the current stream.  A later entry for the same index wins (a re-admitted slot's page 0 of its released row is given
+        again): the scatter gets each index once, since its order among duplicates is undefined."""
+        last = dict(upd)
+        if not last:
+            return
+        d = self.device_ints(list(last) + list(last.values())).view(2, len(last))
+        self.page_table.view(-1).scatter_(0, d[0], d[1].to(torch.int32))
+
+    def device_ints(self, values: list) -> torch.Tensor:
+        """int64 [len(values)] on the cache's device, copied from pinned host memory without a host synchronisation."""
+        h = torch.tensor(values, dtype=torch.int64).pin_memory()
+        return h.to(self.page_table.device, non_blocking=True)
 
     def check_precision(self, p) -> None:
         """The mode and the weights the cache was opened with are still in force (its K/V rows were computed with them)."""
@@ -157,14 +278,15 @@ class SlotDecodeCache:
                 self.has_action_host[b] = True
 
     def state(self) -> tuple:
-        """Copies of the per-slot state (device vectors and host mirror)."""
-        return (tuple(t.clone() for t in (self.len, self.n_valid, self.has_action, self.active, self.action_token)),
-                (list(self.len_host), list(self.has_action_host), list(self.active_host)))
+        """Copies of the per-slot state: device vectors and page table, host mirror and page allocator."""
+        return (tuple(t.clone() for t in (self.len, self.n_valid, self.has_action, self.active, self.action_token, self.page_table)),
+                (list(self.len_host), list(self.has_action_host), list(self.active_host), self.pages.state()))
 
     def restore(self, st: tuple) -> None:
-        for dst, src in zip((self.len, self.n_valid, self.has_action, self.active, self.action_token), st[0]):
+        for dst, src in zip((self.len, self.n_valid, self.has_action, self.active, self.action_token, self.page_table), st[0]):
             dst.copy_(src)
-        self.len_host, self.has_action_host, self.active_host = (list(x) for x in st[1])
+        self.len_host, self.has_action_host, self.active_host = (list(x) for x in st[1][:3])
+        self.pages.restore(st[1][3])
 
 
 def check_cache_append(cache: "DecodeCache", B: int, L: int, E: int, p) -> None:
@@ -192,7 +314,7 @@ def run_block(ctx, p, W, blk: "Block", x32, x16, c16, *, B, L, E, H, omask, chai
     with `chain_ln` the operands are chain_ln(LN2(...)) (next layer's query LayerNorm), with `want16` they are LN2(...) itself.
     With `cache` (DecodeCache or SlotDecodeCache) the L rows are the NEW tokens of each episode and attention runs over the cached
     prefix + themselves.  With `kv_scatter` = (slots int32 [B], cache) and no `cache`, attention is local and the keys / values of
-    sequence j also go to rows slots[j]*Lmax + r of the cache (decoder-only prefill, HFGPT.prefill).
+    sequence j also go to column r of slot slots[j] of the cache (decoder-only prefill, HFGPT.prefill).
 
     ln_1 never runs as a kernel: c_proj's epilogue emits s = attn + x as fp32 + operands together with per-row partial sums, the
     GEGLU GEMM takes the un-normalised s with ln_1 folded into its weights (rstd / mean applied in its epilogue), and the MLP's
@@ -207,16 +329,21 @@ def run_block(ctx, p, W, blk: "Block", x32, x16, c16, *, B, L, E, H, omask, chai
     if cache is None:
         if kv_scatter is not None:
             sl, kc = kv_scatter
-            ctx.slot_kv_scatter(qkv16.hi, qkv16.lo, qkv16.ld, E, 2 * E, B, L, sl, kc.kv_hi[layer], kc.kv_lo[layer], 2 * E, kc.Lmax)
+            if isinstance(kc, SlotDecodeCache):
+                ctx.slot_kv_scatter_paged(qkv16.hi, qkv16.lo, qkv16.ld, E, 2 * E, B, L, sl, kc.kv_hi[layer], kc.kv_lo[layer], 2 * E,
+                                          kc.page_table, kc.pages.n_pages)
+            else:
+                ctx.slot_kv_scatter(qkv16.hi, qkv16.lo, qkv16.ld, E, 2 * E, B, L, sl, kc.kv_hi[layer], kc.kv_lo[layer], 2 * E, kc.Lmax)
         ctx.attention(q=(qkv16.hi, qkv16.lo, qkv16.ld, 0), k=(qkv16.hi, qkv16.lo, qkv16.ld, E), v=(qkv16.hi, qkv16.lo, qkv16.ld, 2 * E),
                       o=(c16.hi, c16.lo, c16.ld, 0), B=B, H=H, Lq=L, Lk=L, D=d, scale=1.0 / math.sqrt(d), causal=True, key_mask=omask,
                       dtype=p.dtype, o8=o8)
-    elif isinstance(cache, SlotDecodeCache):  # every slot at its own length: columns and causal positions from cache.q_pos
-        khi, klo = cache.kv_hi[layer], cache.kv_lo[layer]
-        ctx.slot_kv_append(qkv16.hi, qkv16.lo, qkv16.ld, E, 2 * E, B, L, cache.q_pos, khi, klo, 2 * E, cache.Lmax)
+    elif isinstance(cache, SlotDecodeCache):  # every slot at its own length: columns and causal positions from cache.q_pos, rows
+        # through the page table
+        khi, klo, pt, n_pages = cache.kv_hi[layer], cache.kv_lo[layer], cache.page_table, cache.pages.n_pages
+        ctx.slot_kv_append_paged(qkv16.hi, qkv16.lo, qkv16.ld, E, 2 * E, B, L, cache.q_pos, khi, klo, 2 * E, pt, n_pages)
         ctx.attention(q=(qkv16.hi, qkv16.lo, qkv16.ld, 0), k=(khi, klo, 2 * E, 0), v=(khi, klo, 2 * E, E), o=(c16.hi, c16.lo, c16.ld, 0),
                       B=B, H=H, Lq=L, Lk=cache.Lmax, D=d, scale=1.0 / math.sqrt(d), causal=True, key_mask=cache.mask, dtype=p.dtype, o8=o8,
-                      kv_batch_rows=cache.Lmax, mask_ld=cache.Lmax, q_pos=cache.q_pos)
+                      mask_ld=cache.Lmax, q_pos=cache.q_pos, kv_pages=pt, kv_pool_pages=n_pages)
     else:
         L0 = cache.L
         cache.append_kv(layer, qkv16, L0, L)
@@ -432,16 +559,17 @@ class XAttnGPT(nn.Module):
         self._pos_guard.poll()
         err = self._pos_guard.device_flag(dev)  # a bad prompt position id is reported by the next step
         kv16 = self._prompt_operand(ctx, p, prompt_tokens.float(), prompt_position_ids, False, n, Lp, E, err)
-        idx = torch.tensor(slots, dtype=torch.int64, device=dev)
+        cache.free_slots(slots)  # a re-admitted slot's history pages go back to the pool; its first step takes new ones
+        idx = cache.device_ints(slots)
         for W, dst in zip(self._packed(ctx, p), cache.prompt_kv):
             kv = eng.gemm(ctx, kv16, W["wkv"], p, want16=True)[1]
             for d_t, s_t in ((dst.hi, kv.hi), (dst.lo, kv.lo)):
                 if d_t is not None:
                     d_t.view(cache.S, cache.Lp_cap, -1)[idx, :Lp] = s_t[: n * Lp].view(n, Lp, -1)
-        cache.prompt_mask[idx] = 0
+        cache.prompt_mask.index_fill_(0, idx, 0)
         cache.prompt_mask[idx, :Lp] = prompt_mask_u8
         for t, v in ((cache.len, 0), (cache.n_valid, 0), (cache.has_action, 0), (cache.active, 1)):
-            t[idx] = v
+            t.index_fill_(0, idx, v)
         for b in slots:
             cache.len_host[b], cache.has_action_host[b], cache.active_host[b] = 0, False, True
 
@@ -618,15 +746,20 @@ class HFGPT(nn.Module):
     def prefill(self, cache, slots: list, x: torch.Tensor, custom_mask_u8: torch.Tensor, position_ids: torch.Tensor) -> None:
         """Decoder-only prompt prefill.  x (L,n,E) holds n new sequences [prompt | separator] (custom_mask_u8 / position_ids (n,L);
         the separator, last, is valid).  They run through every block with local causal attention -- the arithmetic of `forward` --
-        and after each layer's c_attn GEMM their keys / values go to cache rows slots[j]*Lmax + r (vima_slot_kv_scatter).  Then the
-        mask columns [0, L) and the state are set: a SlotDecodeCache's by vima_slot_admit_prefix (len = L, n_valid = valid tokens,
-        no action, active), a DecodeCache's (slots = all its rows, in order) by copying the mask and setting L and n_valid.  The
-        caller has validated shapes, slots, capacity and the precision mode."""
+        and after each layer's c_attn GEMM their keys / values go to cache columns [0, L) of slots[j] (vima_slot_kv_scatter; into the
+        pages the slots take first for a SlotDecodeCache, whose earlier pages go back to the pool).  Then the mask columns [0, L)
+        and the state are set: a SlotDecodeCache's by vima_slot_admit_prefix (len = L, n_valid = valid tokens, no action, active), a
+        DecodeCache's (slots = all its rows, in order) by copying the mask and setting L and n_valid.  The caller has validated
+        shapes, slots, capacity (for a SlotDecodeCache also check_prefix) and the precision mode."""
         eng.uses(self)  # fp32 parameters read by the kernels directly
         ctx = eng.ctx_for(x)
         p = eng.prec()
         L, n, E = x.shape
-        sl = torch.tensor(slots, dtype=torch.int32, device=x.device)
+        if isinstance(cache, SlotDecodeCache):
+            cache.free_slots(slots, L)
+            sl = cache.device_ints(slots).to(torch.int32)
+        else:
+            sl = torch.tensor(slots, dtype=torch.int32, device=x.device)
         self._stack(ctx, p, x, custom_mask_u8, position_ids, False, kv_scatter=(sl, cache))
         if isinstance(cache, SlotDecodeCache):
             ctx.slot_admit_prefix(sl, custom_mask_u8[:, :L - 1].contiguous(), cache.Lmax, cache.mask, len_=cache.len, n_valid=cache.n_valid,

@@ -166,9 +166,10 @@ class VIMAGatoPolicy(nn.Module):
     # Slot decode: each row of the batch holds one episode at its own length (VIMAPolicy.open_slots ... capture_step_slots).  A
     # slot's columns [0, Lp+1) hold its prompt and separator; the step kernels are VIMAPolicy's with an all-ones obs mask, so their
     # position rule n_valid + cumsum - 1 is Gato's n_valid + arange.
-    def open_slots(self, n_slots: int, *, max_tokens: Optional[int] = None):
+    def open_slots(self, n_slots: int, *, max_tokens: Optional[int] = None, kv_pool_tokens: Optional[int] = None):
         """Allocate a SlotDecodeCache of `n_slots` slots (all inactive) of `max_tokens` columns each, prompt and separator included
-        (default: the decoder's n_positions), in the current precision mode."""
+        (default: the decoder's n_positions), in the current precision mode, its K/V in a pool of `kv_pool_tokens` tokens
+        (VIMAPolicy.open_slots)."""
         w = self.transformer.lm.positions_embed.weight
         eng.ctx_for(w)
         n_pos = self.transformer.n_positions
@@ -179,7 +180,7 @@ class VIMAGatoPolicy(nn.Module):
             raise ValueError("n_slots must be >= 1")
         p = eng.prec()
         return vnn.SlotDecodeCache(S=int(n_slots), Lmax=Lmax, Lp_cap=0, E=self.embed_dim, n_layer=self.transformer.n_layer, device=w.device,
-                                   split=p.split, precision=p.name, weights=self._decode_weights())
+                                   split=p.split, precision=p.name, weights=self._decode_weights(), kv_pool_tokens=kv_pool_tokens)
 
     def admit(self, cache, slots, prompt_token: torch.Tensor, prompt_token_mask: torch.Tensor) -> None:
         """Start a new episode in each of `slots` (replacing whatever they held): prompt_token (Lp,n,E), prompt_token_mask (n,Lp).
@@ -190,6 +191,7 @@ class VIMAGatoPolicy(nn.Module):
             raise ValueError("admit: this SlotDecodeCache was opened for a cross-attention decoder")
         self._check_prompt(prompt_token, prompt_token_mask, len(s), cache.Lmax)
         cache.check_precision(eng.prec())
+        cache.check_prefix(s, prompt_token.shape[0] + 1)  # prompt + separator, in pages the prefill scatters into
         if not s:
             return
         self.transformer.prefill(cache, s, *self._prompt_prefix(ctx, prompt_token, prompt_token_mask))
@@ -205,6 +207,7 @@ class VIMAGatoPolicy(nn.Module):
         _, S, Q, E = obs_token.shape
         self._check_obs(Q)
         cache.check_step(S, Q, E, eng.prec())
+        cache.reserve_step(Q)
         out = self._slot_step(cache, obs_token, action_token)
         cache.advance_host(Q)
         return out

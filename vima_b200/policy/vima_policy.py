@@ -149,9 +149,12 @@ class VIMAPolicy(nn.Module):
     # --------------------------------------------------------------------------------------------------
     # Slot decode (DESIGN.md 7 (f)1): each row of the batch is a slot holding one episode at a time, so episodes start and finish
     # independently (a vectorised environment resets each of its environments on its own).
-    def open_slots(self, n_slots: int, *, max_tokens: Optional[int] = None, max_prompt_tokens: int = 256):
+    def open_slots(self, n_slots: int, *, max_tokens: Optional[int] = None, max_prompt_tokens: int = 256,
+                   kv_pool_tokens: Optional[int] = None):
         """Allocate a SlotDecodeCache of `n_slots` slots (all inactive) with room for `max_tokens` history tokens (default: the
-        decoder's n_positions) and `max_prompt_tokens` prompt tokens per episode, in the current precision mode."""
+        decoder's n_positions) and `max_prompt_tokens` prompt tokens per episode, in the current precision mode.  The slots' history
+        K/V live in a shared pool of 64-token pages holding `kv_pool_tokens` tokens (default: n_slots * max_tokens, rounded up to
+        whole pages per slot, so every slot can reach max_tokens at once); a smaller pool refuses a step it cannot cover."""
         dev = self.xattn_gpt.positions_embed.weight.device
         eng.ctx_for(self.xattn_gpt.positions_embed.weight)
         Lmax = self.xattn_gpt.n_positions if max_tokens is None else int(max_tokens)
@@ -163,7 +166,8 @@ class VIMAPolicy(nn.Module):
             raise ValueError("n_slots must be >= 1")
         p = eng.prec()
         return vnn.SlotDecodeCache(S=int(n_slots), Lmax=Lmax, Lp_cap=int(max_prompt_tokens), E=self.embed_dim, n_layer=self.xattn_gpt.n_layer,
-                                   device=dev, split=p.split, precision=p.name, weights=eng.WeightState([self.xattn_gpt]))
+                                   device=dev, split=p.split, precision=p.name, weights=eng.WeightState([self.xattn_gpt]),
+                                   kv_pool_tokens=kv_pool_tokens)
 
     def admit(self, cache, slots, prompt_token: torch.Tensor, prompt_token_mask: torch.Tensor) -> None:
         """Start a new episode in each of `slots` (replacing whatever they held): prompt_token (Lp,n,E), prompt_token_mask (n,Lp),
@@ -183,10 +187,12 @@ class VIMAPolicy(nn.Module):
         self.xattn_gpt.admit_prompts(cache, s, prompt_token, pmask_u8, self._prompt_positions(ctx, pmask_u8))
 
     def release(self, cache, slots) -> None:
-        """Mark `slots` inactive (their episodes ended); they keep computing on whatever is passed but never advance."""
+        """Mark `slots` inactive (their episodes ended) and return their K/V pages to the pool; they keep computing on whatever is
+        passed (at column 0, over the zero page) but never advance."""
         s = cache.slot_index(slots)
         if s:
-            cache.active[torch.tensor(s, dtype=torch.int64, device=cache.active.device)] = 0
+            cache.active.index_fill_(0, cache.device_ints(s), 0)
+            cache.free_slots(s)
         for b in s:
             cache.active_host[b] = False
 
@@ -196,6 +202,7 @@ class VIMAPolicy(nn.Module):
         the row equals `forward(...)[-1:]` at B=1 over that episode's own history; an inactive slot's row is unspecified."""
         _, S, Q, E = obs_token.shape
         cache.check_step(S, Q, E, eng.prec())  # every refusal happens before any state is touched
+        cache.reserve_step(Q)
         out = self._slot_step(cache, obs_token, obs_mask, action_token)
         cache.advance_host(Q)
         return out
@@ -244,6 +251,7 @@ class VIMAPolicy(nn.Module):
         S, E = obs_token.shape[1], obs_token.shape[-1]
         Q = obs_token.shape[2] if obs_token.dim() == 4 else 1
         cache.check_step(S, Q, E, eng.prec())
+        cache.reserve_step(Q)
         if "_act_grouped" not in self.__dict__:  # head buffers of its own, apart from forward_action_decoder's (one shape resident)
             self._act_grouped = vnn.action._GroupedMLPs()
         out = self._act_step(cache, *inputs, sampler=sampler, grouped=self._act_grouped)
