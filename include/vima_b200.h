@@ -25,7 +25,7 @@
  *     `vima_sizeof_*()` report the library's own sizes (bindings assert equality at load time).
  *   - the calling thread's current CUDA device is saved and restored around every call.
  *   - environment (read ONCE, in vima_create): VIMA_B200_ATTN = tc (default) | mma;  VIMA_B200_ATTN_TAIL = kernel (default) | off;
- *     VIMA_B200_EPI_PREFETCH = 0 (default) | 1;  VIMA_B200_ATTN_BIAS = auto (default) | tc.
+ *     VIMA_B200_EPI_PREFETCH = 0 (default) | 1;  VIMA_B200_ATTN_BIAS = auto (default) | tc;  VIMA_B200_GEMM_WIDE = 1 (default) | 0.
  */
 #ifndef VIMA_B200_H
 #define VIMA_B200_H
@@ -57,6 +57,9 @@ int vima_sm_count(vima_ctx* ctx);
  * key "attn" = "tc" | "mma";  "attn_tail" = "kernel" | "off" (the <= 8 query rows past the last full 128-row tile: SIMT tail
  * kernel, or one more wgmma tile);
  * "epi_prefetch" = "1" | "0";
+ * "gemm_wide" = "1" | "0" (f16f8 GEMMs whose tiles are 128 wide and N % 256 == 0, with an epilogue of the specialised list: "1" runs
+ * each pair of adjacent tiles as one 128 x 256 tile, a quarter less operand traffic from L2 per multiply-add; results, the GLU
+ * pairing and stats_parts are those of the 128-wide tiles, up to the rounding of the e4m3 cross terms' fp16 sum);
  * "attn_bias" = "auto" | "tc" (relative-bias attention, head_dim 64, non-causal -- the T5 encoder: "auto" runs the K/V-streaming
  * wgmma kernel only where the resident-K/V kernel's shared memory does not fit, "tc" at every length; needs "attn" = "tc").
  * Unknown key/value: VIMA_E_INVALID. */

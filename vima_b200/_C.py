@@ -198,7 +198,8 @@ class Context:
     def set_option(self, key: str, value: str) -> None:
         """Kernel selection of this context: attn = tc | mma, attn_tail = kernel | off, epi_prefetch = 1 | 0, attn_bias = auto | tc
         (relative-bias attention, i.e. the T5 encoder, on the K/V-streaming wgmma kernel only past the resident-K/V kernel's
-        shared memory, or at every length)."""
+        shared memory, or at every length), gemm_wide = 1 | 0 (f16f8 GEMMs with 128-wide tiles and N % 256 == 0 on 128 x 256
+        tiles, or on the 128-wide kernel)."""
         self._ck(self.lib.vima_set_option(self.h, key.encode(), str(value).encode()), "set_option")
 
     @property

@@ -11,8 +11,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT_DIR = os.path.join(HERE, "_lib")
 LIB_PATH = os.path.join(OUT_DIR, "libvima_b200.so")
-SOURCES = ["api.cu", "gemm_tc_f16.cu", "gemm_tc_f16x3.cu", "gemm_tc_f16f8.cu", "gemm_tc_bf16.cu", "gemm_tc_bf16x3.cu", "norm.cu", "attention.cu", "attention_tc.cu", "attention_tc_paged.cu", "attention_tail.cu", "gemm_simt.cu", "misc.cu", "prepare.cu", "slots.cu"]
-HEADERS = ["common.cuh", "kernels.h", "attention_tc.cuh", "gemm_tc.cuh", "gemm_tc_variants.cuh", os.path.join("..", "..", "include", "vima_b200.h")]
+SOURCES = ["api.cu", "gemm_tc_f16.cu", "gemm_tc_f16x3.cu", "gemm_tc_f16f8.cu", "gemm_tc_bf16.cu", "gemm_tc_bf16x3.cu", "gemm_wide_f16f8.cu", "norm.cu", "attention.cu", "attention_tc.cu", "attention_tc_paged.cu", "attention_tail.cu", "gemm_simt.cu", "misc.cu", "prepare.cu", "slots.cu"]
+HEADERS = ["common.cuh", "kernels.h", "attention_tc.cuh", "gemm_tc.cuh", "gemm_tc_variants.cuh", "gemm_wide.cuh", os.path.join("..", "..", "include", "vima_b200.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",

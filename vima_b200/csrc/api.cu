@@ -7,7 +7,7 @@
 #include <cstdlib>
 
 #include "../../include/vima_b200.h"
-#include "gemm_tc_variants.cuh"
+#include "gemm_wide.cuh"
 #include "kernels.h"
 
 using namespace vima;
@@ -27,6 +27,7 @@ struct vima_ctx {
   int epi_prefetch;  // VIMA_B200_EPI_PREFETCH: L2 prefetch of the next tile's residual / multiplier rows (default 0)
   int attn_bias_tc;  // VIMA_B200_ATTN_BIAS: relative-bias attention (T5) on the streaming wgmma kernel: 0 = "auto" (default; only past the
                      // resident-K/V kernel's shared memory), 1 = "tc" (at every length)
+  int gemm_wide;     // VIMA_B200_GEMM_WIDE: f16f8 GEMMs of 128-wide tiles and N % 256 == 0 on gemm_wide_kernel (1, default) | gemm_tc_kernel (0)
 };
 
 // Restores the calling thread's CUDA device when an entry point returns (the library switches to the context's device).
@@ -104,6 +105,8 @@ int vima_set_option(vima_ctx* c, const char* key, const char* value) {
     if (!strcmp(value, "tc")) { c->attn_bias_tc = 1; return VIMA_OK; }
   } else if (!strcmp(key, "epi_prefetch")) {
     if (!strcmp(value, "0") || !strcmp(value, "1")) { c->epi_prefetch = value[0] == '1'; return VIMA_OK; }
+  } else if (!strcmp(key, "gemm_wide")) {
+    if (!strcmp(value, "0") || !strcmp(value, "1")) { c->gemm_wide = value[0] == '1'; return VIMA_OK; }
   }
   return fail(c, VIMA_E_INVALID, "set_option: unknown option %s=%s", key, value);
 }
@@ -131,11 +134,12 @@ int vima_create(vima_ctx** out, int device) {
     return VIMA_E_CUDA;
   }
   c->encode_tiled = fn;
-  c->attn_tc = 1; c->attn_tail = 1; c->epi_prefetch = 0; c->attn_bias_tc = 0;
+  c->attn_tc = 1; c->attn_tail = 1; c->epi_prefetch = 0; c->attn_bias_tc = 0; c->gemm_wide = 1;
   if (const char* e = getenv("VIMA_B200_ATTN")) vima_set_option(c, "attn", e);  // unknown values keep the default
   if (const char* e = getenv("VIMA_B200_ATTN_TAIL")) vima_set_option(c, "attn_tail", e);
   if (const char* e = getenv("VIMA_B200_EPI_PREFETCH")) vima_set_option(c, "epi_prefetch", e);
   if (const char* e = getenv("VIMA_B200_ATTN_BIAS")) vima_set_option(c, "attn_bias", e);
+  if (const char* e = getenv("VIMA_B200_GEMM_WIDE")) vima_set_option(c, "gemm_wide", e);
   c->err[0] = 0;
   *out = c;
   return VIMA_OK;
@@ -266,18 +270,28 @@ int vima_gemm(vima_ctx* c, const vima_gemm_desc* d_in, void* stream) {
   GemmParams p;
   memset(&p, 0, sizeof(p));
   const int split = f8 ? 2 : (d->a_lo != nullptr ? 1 : 0);
+  GemmLaunch l;
+  l.act = d->act; l.glu = d->glu != 0; l.mul = d->mul != nullptr; l.res = d->residual != nullptr;
+  l.o32 = d->out_f32 != nullptr; l.o16 = d->out_hi != nullptr; l.dtype = d->dtype;
+  l.lna = d->row_stats != nullptr; l.lnr = d->res_stats != nullptr; l.stats = d->stats_out != nullptr;
+  l.split = split; l.block_n = bn;
+  // f16f8 GEMMs of 128-wide tiles run as pairs of adjacent tiles on the 128 x 256 kernel (a quarter less operand traffic from L2
+  // per multiply-add); the epilogue, the GLU pairing and the row-statistics parts are those of the 128-wide tiles
+  const bool wide = c->gemm_wide && split == 2 && bn == 128 && d->N % GEMM_WIDE_BN == 0 && gemm_wide_has_epilogue(l) &&
+                    gemm_wide_smem_bytes() <= (size_t)c->max_smem_optin;
+  const int tile_n = wide ? GEMM_WIDE_BN : bn;
   int rc;
-  const int tiles_m_ = (d->M + GEMM_BM - 1) / GEMM_BM, tiles_n_ = (d->N + bn - 1) / bn;
+  const int tiles_m_ = (d->M + GEMM_BM - 1) / GEMM_BM, tiles_n_ = (d->N + tile_n - 1) / tile_n;
   if ((rc = make_tmap(c, &p.tm_a_hi, d->a_hi, d->dtype, d->M, d->K, d->lda, GEMM_BM))) return rc;
-  if ((rc = make_tmap(c, &p.tm_b_hi, d->b_hi, d->dtype, d->N, d->K, d->ldb, bn))) return rc;
+  if ((rc = make_tmap(c, &p.tm_b_hi, d->b_hi, d->dtype, d->N, d->K, d->ldb, tile_n))) return rc;
   if (split == 1) {
     if ((rc = make_tmap(c, &p.tm_a_lo, d->a_lo, d->dtype, d->M, d->K, d->lda, GEMM_BM))) return rc;
     if ((rc = make_tmap(c, &p.tm_b_lo, d->b_lo, d->dtype, d->N, d->K, d->ldb, bn))) return rc;
   } else if (split == 2) {
     if ((rc = make_tmap_f8(c, &p.tm_a_lo, d->a_lo8, d->M, d->K, d->lda8, GEMM_BM))) return rc;
     if ((rc = make_tmap_f8(c, &p.tm_a_hi8, d->a_hi8, d->M, d->K, d->lda8, GEMM_BM))) return rc;
-    if ((rc = make_tmap_f8(c, &p.tm_b_hi8, d->b_hi8, d->N, d->K, d->ldb8, bn))) return rc;
-    if ((rc = make_tmap_f8(c, &p.tm_b_lo, d->b_lo8, d->N, d->K, d->ldb8, bn))) return rc;
+    if ((rc = make_tmap_f8(c, &p.tm_b_hi8, d->b_hi8, d->N, d->K, d->ldb8, tile_n))) return rc;
+    if ((rc = make_tmap_f8(c, &p.tm_b_lo, d->b_lo8, d->N, d->K, d->ldb8, tile_n))) return rc;
   }
   p.M = d->M; p.N = d->N; p.K = d->K;
   p.dtype = d->dtype;
@@ -295,6 +309,9 @@ int vima_gemm(vima_ctx* c, const vima_gemm_desc* d_in, void* stream) {
   p.res_stats = d->res_stats; p.res_gamma = d->res_gamma; p.res_beta = d->res_beta;
   p.stats_out = d->stats_out; p.stats_parts = d->stats_parts;
 
+  const int tiles = tiles_m_ * tiles_n_;
+  const int grid = tiles < c->sm_count ? tiles : c->sm_count;  // persistent: one CTA per SM walks the tiles
+  if (wide) LAUNCHED(c, launch_gemm_wide(p, l, grid, gemm_wide_smem_bytes(), c->max_smem_optin, (cudaStream_t)stream), "gemm_wide_kernel");
   const size_t stage = (size_t)(GEMM_A_TILE_BYTES + bn * 128) * (split ? 2 : 1);
   const size_t fixed = gemm_smem_bytes(bn, split, 0);
   int n_stages = (int)(((size_t)c->max_smem_optin - fixed) / stage);
@@ -302,13 +319,6 @@ int vima_gemm(vima_ctx* c, const vima_gemm_desc* d_in, void* stream) {
   if (n_stages < 2) return fail(c, VIMA_E_UNSUPPORTED, "gemm: not enough shared memory for 2 stages");
   p.n_stages = n_stages;
   const size_t smem = gemm_smem_bytes(bn, split, n_stages);
-  const int tiles = tiles_m_ * tiles_n_;
-  const int grid = tiles < c->sm_count ? tiles : c->sm_count;  // persistent: one CTA per SM walks the tiles
-  GemmLaunch l;
-  l.act = d->act; l.glu = d->glu != 0; l.mul = d->mul != nullptr; l.res = d->residual != nullptr;
-  l.o32 = d->out_f32 != nullptr; l.o16 = d->out_hi != nullptr; l.dtype = d->dtype;
-  l.lna = d->row_stats != nullptr; l.lnr = d->res_stats != nullptr; l.stats = d->stats_out != nullptr;
-  l.split = split; l.block_n = bn;
   // f16f8 (split 2) is fp16-only (checked above)
   auto launch = d->dtype == DT_BF16 ? (split ? launch_gemm_tc<DT_BF16, 1> : launch_gemm_tc<DT_BF16, 0>)
                                     : (split == 2 ? launch_gemm_tc<DT_F16, 2> : split ? launch_gemm_tc<DT_F16, 1> : launch_gemm_tc<DT_F16, 0>);
