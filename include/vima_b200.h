@@ -291,6 +291,14 @@ int vima_slot_kv_scatter_paged(vima_ctx*, const void* qkv_hi, const void* qkv_lo
  * len[b] = Lp+1, n_valid[b] = sum(prompt_mask[j] != 0) + 1, has_action[b] = 0, active[b] = 1.  Lp + 1 <= Lmax. */
 int vima_slot_admit_prefix(vima_ctx*, const int32_t* slots, int n, const uint8_t* prompt_mask, int Lp, int Lmax, uint8_t* slot_mask,
                            int32_t* len, int32_t* n_valid, int32_t* has_action, int32_t* active, void* stream);
+/* Forked slots (no reference counterpart: it runs one episode per call): copy block i of block_rows rows from row src_row0[i] to row
+ * dst_row0[i] in each of n_buf buffers of the same row width -- the copy on write of a shared K/V page (block_rows = 64, every
+ * layer's hi and lo pool) and a fork's prompt K/V rows (block_rows = Lp_cap).  bufs: DEVICE array of n_buf base pointers, each a
+ * buffer of buf_rows rows of row_bytes bytes (row_bytes a positive multiple of 16, bases 16-byte aligned; a null or misaligned
+ * base is skipped); src_row0 / dst_row0: DEVICE int64 [n_blocks].  A block whose start lies outside [0, buf_rows - block_rows]
+ * is skipped, never written.  Destination blocks must not overlap any block's source rows. */
+int vima_kv_copy_blocks(vima_ctx*, void* const* bufs, int n_buf, int64_t row_bytes, const int64_t* src_row0, const int64_t* dst_row0,
+                        int n_blocks, int block_rows, int64_t buf_rows, void* stream);
 /* out[b,l,:] = tok[b*stride_b + l*stride_l + :] + table[ids[b,l]]  (xattn_gpt.py:103-105,110-114); out-of-range
  * ids set *err_flag (device int) to 1 -- the reference raises IndexError there. */
 int vima_add_pos_embed(vima_ctx*, const float* tok, int64_t stride_b, int64_t stride_l, const int64_t* ids, const float* table, int n_pos,

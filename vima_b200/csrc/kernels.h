@@ -204,5 +204,9 @@ cudaError_t launch_slot_kv_scatter(const unsigned short* qkv_hi, const unsigned 
                                    int pool_pages, cudaStream_t s);
 cudaError_t launch_slot_admit_prefix(const int* slots, int n, const unsigned char* prompt_mask, int Lp, int Lmax, unsigned char* slot_mask,
                                      int* len, int* n_valid, int* has_action, int* active, cudaStream_t s);
+// Block i of rows [src_row0[i], +block_rows) -> [dst_row0[i], +block_rows) in each of the n_buf buffers bufs[] (device array),
+// rows of row_bytes (a multiple of 16); blocks with a start outside [0, buf_rows - block_rows] are skipped.
+cudaError_t launch_kv_copy_blocks(void* const* bufs, int n_buf, long long row_bytes, const long long* src_row0, const long long* dst_row0,
+                                  int n_blocks, int block_rows, long long buf_rows, cudaStream_t s);
 
 }  // namespace vima

@@ -196,4 +196,32 @@ cudaError_t launch_slot_admit_prefix(const int* slots, int n, const unsigned cha
   return cudaGetLastError();
 }
 
+// Block copies between rows of the same buffers (copy on write of shared K/V pages, a fork's prompt K/V rows).  Grid (row chunk,
+// block, buffer): block i of buffer z, rows [src_row0[i], +block_rows) -> rows [dst_row0[i], +block_rows), 16 bytes per thread and
+// trip.  The block's rows are contiguous (pitch = row_bytes), so each block is one flat copy.  A block with either start outside
+// [0, buf_rows - block_rows], or a buffer whose base is null or not 16-byte aligned, is skipped.
+__global__ void __launch_bounds__(256) kv_copy_blocks_kernel(void* const* __restrict__ bufs, long long row16,
+                                                             const long long* __restrict__ src_row0, const long long* __restrict__ dst_row0,
+                                                             int n_blocks, int block_rows, long long buf_rows) {
+  uint4* buf = reinterpret_cast<uint4*>(bufs[blockIdx.z]);
+  if (buf == nullptr || (reinterpret_cast<uintptr_t>(buf) & 15)) return;
+  const long long n16 = (long long)block_rows * row16, last = buf_rows - block_rows;
+  for (int i = blockIdx.y; i < n_blocks; i += gridDim.y) {
+    const long long s = __ldg(src_row0 + i), d = __ldg(dst_row0 + i);
+    if (s < 0 || s > last || d < 0 || d > last) continue;
+    const uint4* from = buf + s * row16;
+    uint4* to = buf + d * row16;
+    for (long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x; j < n16; j += (long long)gridDim.x * blockDim.x) to[j] = from[j];
+  }
+}
+
+cudaError_t launch_kv_copy_blocks(void* const* bufs, int n_buf, long long row_bytes, const long long* src_row0, const long long* dst_row0,
+                                  int n_blocks, int block_rows, long long buf_rows, cudaStream_t s) {
+  if (n_blocks == 0) return cudaSuccess;
+  const long long n16 = (long long)block_rows * (row_bytes / 16);
+  const dim3 grid((unsigned)min((n16 + 255) / 256, 1024ll), (unsigned)min(n_blocks, 65535), (unsigned)n_buf);
+  kv_copy_blocks_kernel<<<grid, 256, 0, s>>>(bufs, row_bytes / 16, src_row0, dst_row0, n_blocks, block_rows, buf_rows);
+  return cudaGetLastError();
+}
+
 }  // namespace vima

@@ -99,10 +99,12 @@ class DecodeCache:
 
 
 class KVPagePool:
-    """Host allocator of a paged slot K/V cache (DESIGN.md 7 (f)1): pages 1 .. n_pages-1 of KV_PAGE_TOKENS cache columns each; page 0
-    is the zero page that no slot owns.  `owned[b]` lists the pages of slot b's columns [0, 64*len(owned[b])) in column order, so
-    row b of the page table is owned[b] followed by zeros.  `free` is the free list (taken from its end).  Pure Python: the cache
-    pushes the table entries that each call returns, as (flat index b*page_ld + k, page) pairs."""
+    """Host allocator of a paged slot K/V cache (DESIGN.md 4 and 7 (f)1): pages 1 .. n_pages-1 of KV_PAGE_TOKENS cache columns each;
+    page 0 is the zero page that no slot owns.  `owned[b]` lists the pages of slot b's columns [0, 64*len(owned[b])) in column order,
+    so row b of the page table is owned[b] followed by zeros.  `free` is the free list (taken from its end).  `refs[p]` counts the
+    slots holding page p: a fork shares pages by reference, a page goes back to the free list when its last holder lets it go, and
+    a holder that is about to write into a shared page takes a private copy first (`cow`).  Pure Python: the cache pushes the table
+    entries that each call returns, as (flat index b*page_ld + k, page) pairs."""
 
     def __init__(self, S: int, page_ld: int, n_pages: int):
         if n_pages < 2:
@@ -110,6 +112,7 @@ class KVPagePool:
         self.S, self.page_ld, self.n_pages = S, page_ld, n_pages
         self.free = list(range(n_pages - 1, 0, -1))
         self.owned = [[] for _ in range(S)]
+        self.refs = [0] * n_pages  # refs[0] stays 0: the zero page is never counted
 
     @staticmethod
     def pages_for(cols: int) -> int:
@@ -125,23 +128,69 @@ class KVPagePool:
         upd = []
         for _ in range(self.needed(b, cols)):
             pg = self.free.pop()
+            self.refs[pg] = 1
             upd.append((b * self.page_ld + len(own), pg))
             own.append(pg)
         return upd
 
     def release(self, b: int) -> list:
-        """Return slot b's pages to the free list; its table row goes back to zeros."""
+        """Let go of slot b's pages (each returns to the free list when no other slot holds it); its table row goes back to zeros."""
         own = self.owned[b]
         upd = [(b * self.page_ld + k, 0) for k in range(len(own))]
-        self.free.extend(reversed(own))
+        for pg in reversed(own):
+            self.refs[pg] -= 1
+            if self.refs[pg] == 0:
+                self.free.append(pg)
         self.owned[b] = []
         return upd
 
+    def fork(self, s: int, d: int, n: int) -> list:
+        """Slot d (holding no pages) takes slot s's first n pages by reference; nothing is allocated."""
+        own = self.owned[s][:n]
+        for pg in own:
+            self.refs[pg] += 1
+        self.owned[d] = list(own)
+        return [(d * self.page_ld + k, pg) for k, pg in enumerate(own)]
+
+    def cow_plan(self, cols: list) -> list:
+        """Which of the (slot, column) pairs, visited in the given order, must copy a shared page before writing `column`: the
+        column lies inside a page (col % 64 != 0; at a page boundary the write starts a page of its own) that some later visitor
+        still holds.  So the last holder in visiting order keeps the page in place.  Changes nothing (`cow` does the copies)."""
+        left, out = {}, []
+        for b, col in cols:
+            k = col // _C.KV_PAGE_TOKENS
+            if col % _C.KV_PAGE_TOKENS == 0 or k >= len(self.owned[b]):
+                continue
+            pg = self.owned[b][k]
+            r = left.get(pg, self.refs[pg])
+            if r > 1:
+                left[pg] = r - 1
+                out.append(b)
+        return out
+
+    def cow(self, b: int, col: int) -> tuple:
+        """Give slot b a private copy of the shared page holding column `col` (after cow_plan said so and a free page was checked):
+        returns (table update, (old page, new page)) -- the caller copies the old page's rows into the new one."""
+        k = col // _C.KV_PAGE_TOKENS
+        old, new = self.owned[b][k], self.free.pop()
+        self.refs[old] -= 1
+        self.refs[new] = 1
+        self.owned[b][k] = new
+        return (b * self.page_ld + k, new), (old, new)
+
+    def freed_by(self, slots: list) -> int:
+        """Pages that would return to the free list if every slot of `slots` let go of its pages."""
+        drop = {}
+        for b in slots:
+            for pg in self.owned[b]:
+                drop[pg] = drop.get(pg, 0) + 1
+        return sum(1 for pg, n in drop.items() if self.refs[pg] == n)
+
     def state(self) -> tuple:
-        return list(self.free), [list(o) for o in self.owned]
+        return list(self.free), [list(o) for o in self.owned], list(self.refs)
 
     def restore(self, st: tuple) -> None:
-        self.free, self.owned = list(st[0]), [list(o) for o in st[1]]
+        self.free, self.owned, self.refs = list(st[0]), [list(o) for o in st[1]], list(st[2])
 
 
 class SlotDecodeCache:
@@ -151,7 +200,8 @@ class SlotDecodeCache:
     is the zero page); `page_table` int32 [S, ceil(Lmax/64)] on the device maps column j of slot b to row page_table[b, j//64]*64 +
     j%64 (0 = no page: reads see zeros, writes are skipped), and `pages` (KVPagePool) is its host mirror with the free list.  A slot
     takes pages on the host before each step (check_step / reserve_step, the step's columns [0, len + Q + 1)) and returns them on
-    release or re-admission.  Projected prompt K/V per layer: `prompt_kv[i]` (an Opnd [S*Lp_cap, 2E]) with `prompt_mask` [S, Lp_cap]
+    release or re-admission; `fork` gives a slot another's pages by reference and `reserve_step` copies a shared page before a
+    sharer writes into it (copy on write).  Projected prompt K/V per layer: `prompt_kv[i]` (an Opnd [S*Lp_cap, 2E]) with `prompt_mask` [S, Lp_cap]
     (a shorter prompt's tail columns are masked).  Per-slot device state, int32 [S]: `len` (cache columns used), `n_valid` (next
     position id), `has_action`, `active`; `q_pos` is the step's scratch copy of `len`.  `action_token` fp32 [S, E] is the embedding
     of each slot's last action that `act_slots` feeds back to the next step (zero at open; a slot's first step ignores it).
@@ -184,6 +234,7 @@ class SlotDecodeCache:
         z = lambda: torch.zeros((S,), dtype=torch.int32, device=device)
         self.len, self.n_valid, self.has_action, self.active, self.q_pos = z(), z(), z(), z(), z()
         self.action_token = torch.zeros((S, E), dtype=torch.float32, device=device)
+        self._copy_bufs = {}  # base addresses of the buffers vima_kv_copy_blocks copies rows in, on the device (copy_bufs)
         self.len_host = [0] * S
         self.has_action_host = [False] * S
         self.active_host = [False] * S
@@ -197,9 +248,15 @@ class SlotDecodeCache:
     def kv_pages_free(self) -> int:
         return len(self.pages.free)
 
+    def _cow_plan(self) -> list:
+        """Active slots whose next step writes into a page shared with another slot (a fork's), in ascending slot order."""
+        return self.pages.cow_plan([(b, self.len_host[b]) for b in range(self.S) if self.active_host[b]])
+
     def kv_pages_needed(self, Q: int) -> int:
-        """New pages the next step of Q obs tokens takes: every active slot must own its columns [0, len + Q + 1)."""
-        return sum(self.pages.needed(b, self.len_host[b] + Q + 1) for b in range(self.S) if self.active_host[b])
+        """New pages the next step of Q obs tokens takes: every active slot must own its columns [0, len + Q + 1), and a slot whose
+        column `len` lies inside a page it shares takes a private copy of that page first."""
+        new = sum(self.pages.needed(b, self.len_host[b] + Q + 1) for b in range(self.S) if self.active_host[b])
+        return new + len(self._cow_plan())
 
     def slot_index(self, slots) -> list:
         s = [int(x) for x in (slots.tolist() if isinstance(slots, torch.Tensor) else slots)]
@@ -223,18 +280,41 @@ class SlotDecodeCache:
         self.check_precision(p)
 
     def reserve_step(self, Q: int) -> None:
-        """Take the pages the next step needs (after check_step, so it cannot fail); asynchronous, no host synchronisation."""
-        upd = []
+        """Take the pages the next step needs (after check_step, so it cannot fail): first a private copy of each shared page a slot
+        is about to write into (one vima_kv_copy_blocks over every layer's pool), then the new pages.  Asynchronous, no host
+        synchronisation; the copies are queued on the current stream ahead of the step's kernels."""
+        upd, copies = [], []
+        for b in self._cow_plan():
+            u, c = self.pages.cow(b, self.len_host[b])
+            upd.append(u)
+            copies.append(c)
         for b in range(self.S):
             if self.active_host[b]:
                 upd += self.pages.reserve(b, self.len_host[b] + Q + 1)
+        if copies:
+            self._copy_pages(copies)
         self._push_pages(upd)
+
+    def copy_bufs(self, which: str) -> torch.Tensor:
+        """int64 device array of base addresses: "pool" = every layer's K/V pool, hi and lo (copy on write of a shared page),
+        "prompt" = every layer's prompt K/V, hi and lo (a fork).  Built on first use."""
+        if which not in self._copy_bufs:
+            ts = self.kv_hi + self.kv_lo if which == "pool" else [t for o in self.prompt_kv for t in (o.hi, o.lo)]
+            self._copy_bufs[which] = self.device_ints([t.data_ptr() for t in ts if t is not None])
+        return self._copy_bufs[which]
+
+    def _copy_pages(self, copies: list) -> None:
+        """(old page, new page) pairs: the old page's 64 rows -> the new page's, in every layer's hi and lo pool, one launch."""
+        rows = self.device_ints([old * _C.KV_PAGE_TOKENS for old, _ in copies] + [new * _C.KV_PAGE_TOKENS for _, new in copies])
+        rows = rows.view(2, len(copies))
+        _C.Context.get(self.page_table.device).kv_copy_blocks(self.copy_bufs("pool"), self.kv_hi[0].stride(0) * 2, rows[0], rows[1],
+                                                              _C.KV_PAGE_TOKENS, self.pages.n_pages * _C.KV_PAGE_TOKENS)
 
     def check_prefix(self, slots: list, cols: int) -> None:
         """Refuses (before any state is touched) an admission of `slots` whose first `cols` columns the pool cannot cover, counting
-        the pages the slots give back."""
+        the pages the slots give back (a page still shared with a slot outside `slots` is not given back)."""
         need = len(slots) * self.pages.pages_for(cols)
-        have = self.kv_pages_free + sum(len(self.pages.owned[b]) for b in slots)
+        have = self.kv_pages_free + self.pages.freed_by(slots)
         if need > have:
             raise ValueError(f"admitting {len(slots)} prefixes of {cols} tokens needs {need} K/V pages, {have} are free: release "
                              "slots or open the cache with a larger kv_pool_tokens")
@@ -248,6 +328,46 @@ class SlotDecodeCache:
         for b in slots:
             upd += self.pages.reserve(b, prefix_cols)
         self._push_pages(upd)
+
+    def check_fork(self, src, dst) -> tuple:
+        """Everything that can refuse a fork, before any state is touched: -> (src, dst) as lists of ints."""
+        s = [int(x) for x in (src.tolist() if isinstance(src, torch.Tensor) else src)]
+        d = self.slot_index(dst)
+        if len(s) != len(d):
+            raise ValueError(f"fork: {len(s)} sources for {len(d)} destinations")
+        bad = [x for x in s if not 0 <= x < self.S or not self.active_host[x]]
+        if bad:
+            raise ValueError(f"fork: sources {bad} are not active slots of [0, {self.S})")
+        both = sorted(set(s) & set(d))
+        if both:
+            raise ValueError(f"fork: slots {both} are both a source and a destination")
+        return s, d
+
+    def fork(self, src: list, dst: list) -> None:
+        """Slot dst[i] takes a copy of slot src[i]'s episode (after check_fork): its pages by reference (the pages of the columns
+        [0, len) the source has written; no page is taken), its per-slot state, fed-back action, history mask, prompt mask and
+        prompt K/V rows.  A live destination lets go of its pages first.  Asynchronous, no host synchronisation."""
+        if not dst:
+            return
+        upd = []
+        for b in dst:
+            upd += self.pages.release(b)
+        for a, b in zip(src, dst):
+            upd += self.pages.fork(a, b, self.pages.pages_for(self.len_host[a]))
+        self._push_pages(upd)
+        n = len(dst)
+        idx = self.device_ints(src + dst)
+        si, di = idx[:n], idx[n:]
+        rows = [self.len, self.n_valid, self.has_action, self.active, self.action_token, self.mask]
+        if self.Lp_cap:
+            rows.append(self.prompt_mask)
+            starts = idx * self.Lp_cap
+            _C.Context.get(self.page_table.device).kv_copy_blocks(self.copy_bufs("prompt"), self.prompt_kv[0].hi.stride(0) * 2, starts[:n],
+                                                                  starts[n:], self.Lp_cap, self.S * self.Lp_cap)
+        for t in rows:
+            t.index_copy_(0, di, t.index_select(0, si))
+        for a, b in zip(src, dst):
+            self.len_host[b], self.has_action_host[b], self.active_host[b] = self.len_host[a], self.has_action_host[a], True
 
     def _push_pages(self, upd: list) -> None:
         """Page-table entries (flat index, page) -> the device table: one copy from pinned host memory and one scatter, both queued

@@ -110,6 +110,7 @@ class VIMAFlamingoPolicy(VIMAGatoPolicy):
         return VIMAPolicy.admit(self, cache, slots, prompt_token, prompt_token_mask)
 
     release = VIMAPolicy.release
+    fork_slots = VIMAPolicy.fork_slots
 
     def step_slots(self, cache, obs_token: torch.Tensor, action_token: Optional[torch.Tensor]) -> torch.Tensor:
         """obs_token (1,S,Q,E), action_token (1,S,E) | None -> (1,S,E), as VIMAPolicy.step_slots with every obs token valid."""

@@ -197,6 +197,7 @@ class VIMAGatoPolicy(nn.Module):
         self.transformer.prefill(cache, s, *self._prompt_prefix(ctx, prompt_token, prompt_token_mask))
 
     release = VIMAPolicy.release
+    fork_slots = VIMAPolicy.fork_slots
     refresh_weights = VIMAPolicy.refresh_weights
 
     def step_slots(self, cache, obs_token: torch.Tensor, action_token: Optional[torch.Tensor]) -> torch.Tensor:

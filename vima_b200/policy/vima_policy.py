@@ -196,6 +196,18 @@ class VIMAPolicy(nn.Module):
         for b in s:
             cache.active_host[b] = False
 
+    def fork_slots(self, cache, src, dst) -> None:
+        """Copy episodes between slots: after the call slot dst[i] holds slot src[i]'s episode exactly as it stands (its history,
+        prompt, fed-back action and state), so the two continue from the same point; a source may repeat, a live destination's
+        episode is replaced.  The history K/V pages are shared by reference and copied only when a sharer next writes into a
+        partly filled one, so a fork takes no page and the pool never refuses it.  Group sampling: admit once, then
+        `fork_slots(cache, [s] * (k - 1), others)` and `act_slots(..., sampler=...)`.  Refuses (ValueError, nothing touched) an
+        inactive or out-of-range source, repeated destinations, a slot that is both, and a cache of another precision mode or of
+        changed weights.  Queued on the current stream, no host synchronisation."""
+        s, d = cache.check_fork(src, dst)
+        cache.check_precision(eng.prec())
+        cache.fork(s, d)
+
     def step_slots(self, cache, obs_token: torch.Tensor, obs_mask: torch.Tensor, action_token: Optional[torch.Tensor]) -> torch.Tensor:
         """One environment step of every slot: obs_token (1,S,Q,E), obs_mask (1,S,Q), action_token (1,S,E) (the previous action of
         each slot; ignored for slots at their first step; None = all zeros) -> predicted action token (1,S,E).  For an active slot
