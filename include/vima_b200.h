@@ -224,14 +224,20 @@ typedef struct {
   /* ---- v5 end ---- */
   /* v6 tail (an addition; the ABI version stays 5): paged k / v (slot decode).  DEVICE int32 [B, kv_page_ld] or NULL.  When set,
    * key j of batch element b is row kv_pages[b*kv_page_ld + j/64]*64 + j%64 of k / v, a pool of kv_pool_pages 64-row pages
-   * (kv_batch_rows is ignored); an entry outside [0, kv_pool_pages) reads page 0.  Needs q_pos, no rel_bias,
-   * Lk <= kv_page_ld*64 and kv_pool_pages*64 < 2^31. */
+   * (kv_batch_rows is ignored); an entry outside [0, kv_pool_pages) reads page 0.  Needs q_pos or non-causal attention, no
+   * rel_bias, Lk <= kv_page_ld*64 and kv_pool_pages*64 < 2^31.  Every kernel reads whole pages: rows of a page past the keys a call
+   * attends must hold finite values (a slot cache keeps them zero). */
   const int32_t* kv_pages;
   int kv_page_ld, kv_pool_pages;
+  /* v7 tail (an addition; the ABI version stays 5): per-batch key count (slot decode's cross-attention over prompts of different
+   * lengths).  DEVICE int32 [B] or NULL.  When set, batch element b attends keys [0, clamp(kv_len[b], 1, Lk)); keys past that count
+   * are excluded like keys past Lk (and whole 64-key chunks past it are never read).  Non-causal only, without q_pos or rel_bias. */
+  const int32_t* kv_len;
 } vima_attn_desc;
 #define VIMA_ATTN_DESC_V4_SIZE offsetof(vima_attn_desc, q_pos)
 #define VIMA_ATTN_DESC_V5_SIZE offsetof(vima_attn_desc, kv_pages)
-#define VIMA_ATTN_DESC_V6_SIZE sizeof(vima_attn_desc)
+#define VIMA_ATTN_DESC_V6_SIZE offsetof(vima_attn_desc, kv_len)
+#define VIMA_ATTN_DESC_V7_SIZE sizeof(vima_attn_desc)
 #define VIMA_KV_PAGE_TOKENS 64 /* rows of one K/V page: the streaming attention kernel's key chunk */
 int vima_attention(vima_ctx*, const vima_attn_desc* d, void* stream);
 

@@ -3,7 +3,9 @@
 Environment: AB_B episodes, AB_L history keys (causal self-attention, Lq = Lk = L), AB_LP cross-attention keys (prompt tokens, Lq = L),
 AB_LQ > 0 adds a decode case (AB_LQ new query rows over AB_L cached keys, queries last), AB_SPLIT formats, AB_MASKED.
 --paged: the decode case also runs as slot decode does (per-element q_pos), from contiguous K/V and from a pool of 64-row pages
-through a shuffled page table (seed 0), both printed (e.g. AB_LQ=33 AB_L=1024 python tools/attn_bench.py --paged).
+through a shuffled page table (seed 0), both printed (e.g. AB_LQ=33 AB_L=1024 python tools/attn_bench.py --paged).  --paged also
+adds the slot step's cross-attention (AB_XQ = 33 query rows per slot over AB_LP prompt keys), timed three ways: contiguous, paged through
+a shuffled page table, and paged with ragged per-slot key counts (kv_len uniform in 1..AB_LP, seed 0) as prompts of different lengths.
 """
 import sys, os, math
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -14,6 +16,8 @@ B, H, D, L, Lp = int(os.environ.get("AB_B", 256)), 24, 32, int(os.environ.get("A
 Ld = int(os.environ.get("AB_LQ", 0))
 E = H * D
 cases = [("self causal", L, L, True), ("cross", L, Lp, False)] + ([(f"decode Lq={Ld}", Ld, L, True)] if Ld > 0 else [])
+if "--paged" in sys.argv:
+    cases.append(("slot cross", int(os.environ.get("AB_XQ", 33)), Lp, False))
 for split in [int(x) for x in os.environ.get("AB_SPLIT", "0,1").split(",")]:
     for name, Lq, Lk, causal in cases:
         mk = lambda r, c: torch.randint(-3000, 3000, (r, c), dtype=torch.int16, device="cuda")
@@ -62,6 +66,28 @@ for split in [int(x) for x in os.environ.get("AB_SPLIT", "0,1").split(",")]:
                 for _ in range(20): ctx.attention(**{**base, **extra})
                 e1.record(); torch.cuda.synchronize()
                 timed.append((" " + label, e0.elapsed_time(e1) / 20))
+        if name == "slot cross":  # the prompt K/V as the slot cache keeps it: 64-row pages of a pool, prompt_len keys per slot
+            pl = -(-Lk // 64)
+            perm = torch.randperm(B * pl, generator=torch.Generator().manual_seed(0)).to(torch.int32) + 1
+            table = perm.view(B, pl).cuda()
+            rows = (table.long()[:, torch.arange(Lk) // 64] * 64 + torch.arange(Lk, device="cuda") % 64).view(-1)
+            pool = torch.zeros((B * pl + 1) * 64, 2 * E, dtype=torch.int16, device="cuda")
+            pool_lo = torch.zeros_like(pool) if split else None
+            pool[rows] = kv
+            if split:
+                pool_lo[rows] = kl
+            full = torch.full((B,), Lk, dtype=torch.int32, device="cuda")
+            ragged = torch.randint(1, Lk + 1, (B,), generator=torch.Generator().manual_seed(0), dtype=torch.int32).cuda()
+            paged = dict(kw, k=(pool, pool_lo, 2 * E, 0), v=(pool, pool_lo, 2 * E, E), kv_pages=table, kv_pool_pages=B * pl + 1)
+            timed = []
+            for label, args in (("contiguous", kw), ("paged", dict(paged, kv_len=full)), ("paged ragged kv_len", dict(paged, kv_len=ragged))):
+                ctx.attention(**args); torch.cuda.synchronize()
+                e0.record()
+                for _ in range(20): ctx.attention(**args)
+                e1.record(); torch.cuda.synchronize()
+                timed.append((" " + label, e0.elapsed_time(e1) / 20))
+            print(f"split={split} slot cross: ragged kv_len mean {ragged.float().mean().item():.1f} of {Lk} keys (the FLOP/s below count all {Lk})",
+                  flush=True)
         # causal: the cached keys in full plus half the square of the new rows (half of Lq * Lk for Lq = Lk)
         pairs = Lq * (Lk - Lq) + Lq * Lq / 2 if causal else Lq * Lk
         fl = 4.0 * B * H * pairs * D

@@ -11,8 +11,10 @@ eager (act_slots) and replayed from one CUDA graph (capture_act_slots), alternat
 Sizes: cfg3 (VIMA-200M, Q = 32 obs tokens, Lp = 256, f16f8) and cfg5 shapes (VIMA-Gato-200M, Q = 16, Lp = 256: 257 prefill rows in
 the self-attention cache).  Reported per run: env-steps/s, admission time per episode (CUDA events around the admit / fork calls,
 on the stream the steps run on), peak K/V pages in use, and the smallest pool the arm's schedule fits (the host allocator's peak,
-read after each step's reservation).  Weights are random (timing only).  Prints the GPU's name and power limit beside the
-numbers, one JSON line per run.
+read after each step's reservation); for cfg3 also the peak prompt pages and the smallest prompt pool (the fork arm's forks share
+their source's prompt pages), and torch.cuda.max_memory_allocated over the run.  --prompt-pool-tokens opens cfg3's caches with that
+prompt pool (default: room for a full-length prompt in every slot).  Weights are random (timing only).  Prints the GPU's name and
+power limit beside the numbers, one JSON line per run.
 """
 import argparse
 import json
@@ -58,7 +60,7 @@ def run_size(size, a, info):
     pmask = torch.ones(n_blocks, Lp, dtype=torch.bool, device="cuda")
     extra = (msk,) if vima else ()
     if vima:
-        open_slots = lambda: pol.open_slots(S, max_tokens=Lmax, max_prompt_tokens=Lp)  # noqa: E731
+        open_slots = lambda: pol.open_slots(S, max_tokens=Lmax, max_prompt_tokens=Lp, prompt_pool_tokens=a.prompt_pool_tokens)  # noqa: E731
     else:
         open_slots = lambda: pol.open_slots(S, max_tokens=Lmax)  # noqa: E731
     print(f"# {info}; {size} ({type(pol).__name__}), {S} slots in groups of {k}, Q={Q}, Lp={Lp}, {a.precision}; {a.groups} groups "
@@ -76,7 +78,7 @@ def run_size(size, a, info):
     def run(cache, arm, step):
         queue = list(range(a.groups))
         remaining = [0] * S
-        ticks, idle_blocks, peak, admits = 0, list(range(n_blocks)), 0, []
+        ticks, idle_blocks, peak, peak_p, admits = 0, list(range(n_blocks)), 0, 0, []
         while True:
             take = idle_blocks[:len(queue)]
             if take:
@@ -85,6 +87,7 @@ def run_size(size, a, info):
                 start_groups(cache, arm, take)
                 ev[1].record()
                 admits.append((ev, len(take) * k))
+                peak_p = max(peak_p, cache.prompt_pages_total - cache.prompt_pages_free)
                 for j in take:
                     for i, n in enumerate(lengths[queue.pop(0)]):
                         remaining[j * k + i] = n
@@ -104,7 +107,7 @@ def run_size(size, a, info):
             idle_blocks = [j for j in range(n_blocks) if not any(remaining[j * k:(j + 1) * k])]
         torch.cuda.synchronize()
         adm_ms = sum(e[0].elapsed_time(e[1]) for e, _ in admits)
-        return ticks, peak, adm_ms, sum(n for _, n in admits)
+        return ticks, peak, peak_p, adm_ms, sum(n for _, n in admits)
 
     with torch.no_grad():
         c = open_slots()  # warm-up: modules, weight packing, kernel attributes
@@ -132,13 +135,16 @@ def run_size(size, a, info):
                         pol.release(cache, list(range(S)))
                         step = lambda c, o: gs(o, *extra)  # noqa: E731
                     torch.cuda.synchronize()
+                    torch.cuda.reset_peak_memory_stats()
                     t0 = time.perf_counter()
-                    ticks, peak, adm_ms, n_adm = run(cache, arm, step)
+                    ticks, peak, peak_p, adm_ms, n_adm = run(cache, arm, step)
                     dt = time.perf_counter() - t0
                     r = {"size": size, "slots": S, "group": k, "arm": arm, "mode": mode, "round": rnd, "seconds": round(dt, 4),
                          "ticks": ticks, "env_steps_per_s": round(total_steps / dt, 1), "ms_per_tick": round(dt * 1e3 / ticks, 3),
                          "admission_ms_per_episode": round(adm_ms / n_adm, 4), "peak_pages": peak, "min_pool_tokens": peak * 64,
-                         "pool_pages_default": cache.kv_pages_total}
+                         "pool_pages_default": cache.kv_pages_total, "max_memory_allocated_gb": round(torch.cuda.max_memory_allocated() / 1e9, 3)}
+                    if vima:
+                        r.update({"peak_prompt_pages": peak_p, "min_prompt_pool_tokens": peak_p * 64, "prompt_pool_pages": cache.prompt_pages_total})
                     r.update(info_run)
                     r["gpu"] = info
                     print(json.dumps(r), flush=True)
@@ -159,6 +165,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=2)
     ap.add_argument("--precision", default="f16f8")
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--prompt-pool-tokens", type=int, default=None, help="cfg3: prompt pool size (default: every slot a full prompt)")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("group_rollout_bench needs a CUDA device")

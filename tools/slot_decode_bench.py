@@ -130,9 +130,14 @@ def main():
     pool_pages = S * page_ld if a.kv_pool_tokens is None else -(-a.kv_pool_tokens // 64)
     pool_bytes = n_layer * (pool_pages + 1) * 64 * 2 * E * 4  # the slot runs' page pool, zero page included
     sched = pages_per_tick(lengths, S, Q, prefix)
+    # cross-attention policies: the projected prompt K/V in their own pool (default size: a full prompt in every slot)
+    prompt_pages = S * -(-Lp // 64)
+    prompt_pool = (f", prompt pool {prompt_pages} pages = {n_layer * (prompt_pages + 1) * 64 * 2 * E * 4 / 1e9:.2f} GB"
+                   if a.policy in ("vima", "flamingo") else "")
     print(f"# {info}; {name}model {a.model or '200M'}, {S} slots, Q={Q}, Lp={Lp}, {a.precision}; {a.episodes} episodes of 1..{a.max_steps} steps "
           f"({total_steps} env-steps, seed {a.seed}); {Lmax} cache columns per slot, K/V cache {kv_bytes / 1e9:.2f} GB unpaged (S*Lmax), "
-          f"page pool {pool_pages} pages = {pool_bytes / 1e9:.2f} GB; the schedule's peak {max(sched)} pages, mean {sum(sched) / len(sched):.0f}")
+          f"page pool {pool_pages} pages = {pool_bytes / 1e9:.2f} GB{prompt_pool}; the schedule's peak {max(sched)} pages, mean "
+          f"{sum(sched) / len(sched):.0f}")
 
     if vima:
         forward_step, step_slots = pol.forward_step, pol.step_slots

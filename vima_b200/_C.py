@@ -86,6 +86,8 @@ class AttnDesc(C.Structure):
         ("q_pos", c_void_p),
         # v6 tail (ABI version 5): paged k / v
         ("kv_pages", c_void_p), ("kv_page_ld", c_int), ("kv_pool_pages", c_int),
+        # v7 tail (ABI version 5): per-batch key count
+        ("kv_len", c_void_p),
     ]
 
 
@@ -294,11 +296,12 @@ class Context:
         self._ck(self.lib.vima_norm(self.h, C.byref(d), c_void_p(self._s())), "norm")
 
     def attention(self, *, q, k, v, o, B, H, Lq, Lk, D, scale, causal=False, key_mask=None, rel_bias=None, dtype=DT_F16, o8=None,
-                  kv_batch_rows=0, mask_ld=0, q_pos0=0, q_pos=None, kv_pages=None, kv_pool_pages=0):
+                  kv_batch_rows=0, mask_ld=0, q_pos0=0, q_pos=None, kv_pages=None, kv_pool_pages=0, kv_len=None):
         """q, k, v, o: (hi, lo|None, ld, column offset) tuples over 16-bit operand buffers.  q_pos: int32 [B] on the device, the
         causal position of each batch element's first query row (its key count is then q_pos[b] + Lq; Lk is the capacity).
         kv_pages: int32 [B, page_ld] on the device, paged k / v: key j of element b is row kv_pages[b, j // 64] * 64 + j % 64 of k / v,
-        a pool of kv_pool_pages pages."""
+        a pool of kv_pool_pages pages.  kv_len: int32 [B] on the device (non-causal, no q_pos): element b attends keys
+        [0, clamp(kv_len[b], 1, Lk))."""
         es = 2
 
         def at(t, off):
@@ -320,6 +323,9 @@ class Context:
         if kv_pages is not None:
             assert kv_pages.dtype == torch.int32 and kv_pages.dim() == 2 and kv_pages.is_contiguous() and kv_pages.shape[0] >= B
             d.kv_pages, d.kv_page_ld, d.kv_pool_pages = kv_pages.data_ptr(), kv_pages.shape[1], int(kv_pool_pages)
+        if kv_len is not None:
+            assert kv_len.dtype == torch.int32 and kv_len.is_contiguous() and kv_len.numel() >= B
+            d.kv_len = kv_len.data_ptr()
         if o8 is not None:  # (lo8, hi8) uint8 [rows, ld8]
             d.o_lo8, d.o_hi8, d.ldo8 = o8[0].data_ptr(), o8[1].data_ptr(), o8[0].stride(0)
         self._ck(self.lib.vima_attention(self.h, C.byref(d), c_void_p(self._s())), "attention")

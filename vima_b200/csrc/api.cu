@@ -397,11 +397,14 @@ int vima_attention(vima_ctx* c, const vima_attn_desc* d_in, void* stream) {
   p.kv_batch_rows = d->kv_batch_rows; p.mask_ld = d->mask_ld; p.q_pos0 = d->q_pos0; p.q_batch_rows = 0;
   p.q_pos = d->q_pos;
   p.kv_pages = d->kv_pages; p.kv_page_ld = d->kv_page_ld; p.kv_pool_pages = d->kv_pool_pages;
-  if (d->kv_pages && (!d->q_pos || d->rel_bias || d->kv_page_ld < 1 || d->kv_pool_pages < 1 || d->Lk > (long long)d->kv_page_ld * VIMA_KV_PAGE_TOKENS ||
-                      (long long)d->kv_pool_pages * VIMA_KV_PAGE_TOKENS > 0x7fffffffll))
-    return fail(c, VIMA_E_INVALID, "attention: paged k / v need q_pos, no relative bias, Lk <= kv_page_ld*%d (Lk %d, kv_page_ld %d) and "
-                "1 <= kv_pool_pages with kv_pool_pages*%d rows inside the 32-bit row range (kv_pool_pages %d)", VIMA_KV_PAGE_TOKENS, d->Lk,
-                d->kv_page_ld, VIMA_KV_PAGE_TOKENS, d->kv_pool_pages);
+  p.kv_len = d->kv_len;
+  if (d->kv_pages && ((d->causal && !d->q_pos) || d->rel_bias || d->kv_page_ld < 1 || d->kv_pool_pages < 1 ||
+                      d->Lk > (long long)d->kv_page_ld * VIMA_KV_PAGE_TOKENS || (long long)d->kv_pool_pages * VIMA_KV_PAGE_TOKENS > 0x7fffffffll))
+    return fail(c, VIMA_E_INVALID, "attention: paged k / v need q_pos (or non-causal attention), no relative bias, Lk <= kv_page_ld*%d (Lk %d, "
+                "kv_page_ld %d) and 1 <= kv_pool_pages with kv_pool_pages*%d rows inside the 32-bit row range (kv_pool_pages %d)",
+                VIMA_KV_PAGE_TOKENS, d->Lk, d->kv_page_ld, VIMA_KV_PAGE_TOKENS, d->kv_pool_pages);
+  if (d->kv_len && (d->causal || d->q_pos || d->rel_bias))
+    return fail(c, VIMA_E_INVALID, "attention: per-batch kv_len needs non-causal attention without q_pos or relative bias");
   if ((d->kv_batch_rows && d->kv_batch_rows < d->Lk) || (d->mask_ld && d->mask_ld < d->Lk) || d->q_pos0 < 0)
     return fail(c, VIMA_E_INVALID, "attention: kv_batch_rows / mask_ld must cover Lk, q_pos0 >= 0");
   if (d->q_pos && (!d->causal || d->rel_bias || d->Lq > d->Lk))

@@ -39,6 +39,7 @@ struct AttnParams {
   // paged k / v (slot decode): key j of batch element b is row kv_pages[b*kv_page_ld + j/64]*64 + j%64 of a pool of kv_pool_pages
   // pages; null = the contiguous layout above
   const int* kv_pages; int kv_page_ld; int kv_pool_pages;
+  const int* kv_len;                           // non-causal, no q_pos (device, or null): batch element b attends keys [0, kv_len[b])
 };
 constexpr int KV_PAGE_TOKENS = 64;  // = the streaming kernel's key chunk: one chunk is one page
 // k / v row of key j of batch element b.  A page entry outside [0, kv_pool_pages) reads as page 0 (the pool's zero page), so no
@@ -64,11 +65,12 @@ __device__ __forceinline__ float attn_key_mask_term(const AttnParams& p, int b, 
   return m;
 }
 // Causal position of query row 0 and key count of batch element b.  With q_pos the key count is q_pos[b] + (full query count of the
-// call; q_batch_rows when a body / tail split gave this launch only part of the rows), clamped to the capacity Lk.
+// call; q_batch_rows when a body / tail split gave this launch only part of the rows), clamped to the capacity Lk; with kv_len it is
+// kv_len[b] clamped to [1, Lk].  Keys past the count are excluded like keys past Lk, and their chunks are not streamed.
 __device__ __forceinline__ void attn_batch_keys(const AttnParams& p, int b, int qbr, int& qp0, int& lk) {
   if (p.q_pos == nullptr) {
     qp0 = p.q_pos0;
-    lk = p.Lk;
+    lk = p.kv_len == nullptr ? p.Lk : min(max(__ldg(p.kv_len + b), 1), p.Lk);
   } else {
     qp0 = max(p.q_pos[b], 0);
     lk = max(min(qp0 + qbr, p.Lk), 1);

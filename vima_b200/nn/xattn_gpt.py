@@ -201,20 +201,31 @@ class SlotDecodeCache:
     j%64 (0 = no page: reads see zeros, writes are skipped), and `pages` (KVPagePool) is its host mirror with the free list.  A slot
     takes pages on the host before each step (check_step / reserve_step, the step's columns [0, len + Q + 1)) and returns them on
     release or re-admission; `fork` gives a slot another's pages by reference and `reserve_step` copies a shared page before a
-    sharer writes into it (copy on write).  Projected prompt K/V per layer: `prompt_kv[i]` (an Opnd [S*Lp_cap, 2E]) with `prompt_mask` [S, Lp_cap]
-    (a shorter prompt's tail columns are masked).  Per-slot device state, int32 [S]: `len` (cache columns used), `n_valid` (next
-    position id), `has_action`, `active`; `q_pos` is the step's scratch copy of `len`.  `action_token` fp32 [S, E] is the embedding
-    of each slot's last action that `act_slots` feeds back to the next step (zero at open; a slot's first step ignores it).
+    sharer writes into it (copy on write).
+
+    Projected prompt K/V per layer (cross-attention models, Lp_cap > 0): `prompt_kv_hi[i]` / `prompt_kv_lo[i]`, a second pool of
+    `prompt_pages_total + 1` pages [(P_p+1)*64, 2E] with its own table `prompt_page_table` int32 [S, ceil(Lp_cap/64)] and host mirror
+    `prompt_pages` (a second KVPagePool), `prompt_len` int32 [S] (the admitted prompt's length: the cross-attention's per-slot key
+    count) and `prompt_mask` [S, Lp_cap] (a shorter prompt's tail columns are masked).  An admission takes ceil(Lp/64) pages per slot
+    and writes them once; the rows of the last page past Lp are zero.  A fork shares the source's prompt pages by reference (prompt
+    pages are never written after admission, so they need no copy on write); release and re-admission give them back.  The two
+    pools have separate budgets: `kv_pages_*` count history pages only.
+
+    Per-slot device state, int32 [S]: `len` (cache columns used), `n_valid` (next position id), `has_action`, `active`; `q_pos` is
+    the step's scratch copy of `len`.  `action_token` fp32 [S, E] is the embedding of each slot's last action that `act_slots` feeds back to the next step (zero at open; a slot's first step ignores it).
     The host mirrors len / has_action / active (it knows them from admissions and the step width), so capacity and pages are
     checked and allocated without reading the device.  A decoder-only model (HFGPT) opens it with Lp_cap = 0: its prompt and
-    separator are the first columns of the self-attention cache (HFGPT.prefill), and there is no prompt_kv / prompt_mask.
+    separator are the first columns of the self-attention cache (HFGPT.prefill), and there is no prompt pool / prompt_mask.
 
     kv_pool_tokens: cache columns the pool holds across all slots (rounded up to pages); None = S*ceil(Lmax/64) pages, so that
     every slot can reach Lmax at once.  A smaller pool overcommits: a step or admission the free pages cannot cover raises
-    ValueError before any state is touched (`kv_pages_needed` tells a driver how many the next step takes)."""
+    ValueError before any state is touched (`kv_pages_needed` tells a driver how many the next step takes).  prompt_pool_tokens:
+    the same for the prompt pool; None = S*ceil(Lp_cap/64) pages, so that every slot can hold a full-length prompt at once."""
+
+    Lp_cap = 0  # prompt columns per slot; 0 = no prompt pool (also for host-side stand-ins that only set up the history pool)
 
     def __init__(self, *, S: int, Lmax: int, Lp_cap: int, E: int, n_layer: int, device, split: bool, precision: str, weights=None,
-                 kv_pool_tokens: Optional[int] = None):
+                 kv_pool_tokens: Optional[int] = None, prompt_pool_tokens: Optional[int] = None):
         self.S, self.Lmax, self.Lp_cap, self.E, self.precision = S, Lmax, Lp_cap, E, precision
         self.weights = weights  # engine.WeightState of the decoder at open; admit and step refuse once it has changed
         page_ld = KVPagePool.pages_for(Lmax)
@@ -222,16 +233,29 @@ class SlotDecodeCache:
         if not 1 <= n_use <= S * page_ld:
             raise ValueError(f"kv_pool_tokens={kv_pool_tokens} must cover 1 .. {S * page_ld} pages of {_C.KV_PAGE_TOKENS} tokens "
                              f"({S} slots of max_tokens={Lmax})")
+        if Lp_cap:
+            p_ld = KVPagePool.pages_for(Lp_cap)
+            n_prompt = S * p_ld if prompt_pool_tokens is None else KVPagePool.pages_for(int(prompt_pool_tokens))
+            if not 1 <= n_prompt <= S * p_ld:
+                raise ValueError(f"prompt_pool_tokens={prompt_pool_tokens} must cover 1 .. {S * p_ld} pages of {_C.KV_PAGE_TOKENS} "
+                                 f"tokens ({S} slots of max_prompt_tokens={Lp_cap})")
         self.pages = KVPagePool(S, page_ld, n_use + 1)
         self.page_table = torch.zeros((S, page_ld), dtype=torch.int32, device=device)
         mk = lambda rows: torch.zeros((rows, 2 * E), dtype=torch.int16, device=device)
         rows = self.pages.n_pages * _C.KV_PAGE_TOKENS
         self.kv_hi = [mk(rows) for _ in range(n_layer)]
         self.kv_lo = [mk(rows) if split else None for _ in range(n_layer)]
-        self.prompt_kv = [eng.Opnd(S * Lp_cap, 2 * E, device, split, zero=True) for _ in range(n_layer)] if Lp_cap else None
-        self.prompt_mask = torch.zeros((S, Lp_cap), dtype=torch.uint8, device=device) if Lp_cap else None
-        self.mask = torch.zeros((S, Lmax), dtype=torch.uint8, device=device)
         z = lambda: torch.zeros((S,), dtype=torch.int32, device=device)
+        self.prompt_pages = self.prompt_page_table = self.prompt_kv_hi = self.prompt_kv_lo = self.prompt_len = self.prompt_mask = None
+        if Lp_cap:
+            self.prompt_pages = KVPagePool(S, p_ld, n_prompt + 1)
+            self.prompt_page_table = torch.zeros((S, p_ld), dtype=torch.int32, device=device)
+            rows = self.prompt_pages.n_pages * _C.KV_PAGE_TOKENS
+            self.prompt_kv_hi = [mk(rows) for _ in range(n_layer)]
+            self.prompt_kv_lo = [mk(rows) if split else None for _ in range(n_layer)]
+            self.prompt_len = z()
+            self.prompt_mask = torch.zeros((S, Lp_cap), dtype=torch.uint8, device=device)
+        self.mask = torch.zeros((S, Lmax), dtype=torch.uint8, device=device)
         self.len, self.n_valid, self.has_action, self.active, self.q_pos = z(), z(), z(), z(), z()
         self.action_token = torch.zeros((S, E), dtype=torch.float32, device=device)
         self._copy_bufs = {}  # base addresses of the buffers vima_kv_copy_blocks copies rows in, on the device (copy_bufs)
@@ -247,6 +271,15 @@ class SlotDecodeCache:
     @property
     def kv_pages_free(self) -> int:
         return len(self.pages.free)
+
+    @property
+    def prompt_pages_total(self) -> int:
+        """Pages of the prompt pool the slots can own (0 without cross-attention prompts)."""
+        return self.prompt_pages.n_pages - 1 if self.Lp_cap else 0
+
+    @property
+    def prompt_pages_free(self) -> int:
+        return len(self.prompt_pages.free) if self.Lp_cap else 0
 
     def _cow_plan(self) -> list:
         """Active slots whose next step writes into a page shared with another slot (a fork's), in ascending slot order."""
@@ -297,9 +330,9 @@ class SlotDecodeCache:
 
     def copy_bufs(self, which: str) -> torch.Tensor:
         """int64 device array of base addresses: "pool" = every layer's K/V pool, hi and lo (copy on write of a shared page),
-        "prompt" = every layer's prompt K/V, hi and lo (a fork).  Built on first use."""
+        "prompt" = every layer's prompt pool, hi and lo (zeroing an admitted prompt's last page).  Built on first use."""
         if which not in self._copy_bufs:
-            ts = self.kv_hi + self.kv_lo if which == "pool" else [t for o in self.prompt_kv for t in (o.hi, o.lo)]
+            ts = self.kv_hi + self.kv_lo if which == "pool" else self.prompt_kv_hi + self.prompt_kv_lo
             self._copy_bufs[which] = self.device_ints([t.data_ptr() for t in ts if t is not None])
         return self._copy_bufs[which]
 
@@ -310,24 +343,51 @@ class SlotDecodeCache:
         _C.Context.get(self.page_table.device).kv_copy_blocks(self.copy_bufs("pool"), self.kv_hi[0].stride(0) * 2, rows[0], rows[1],
                                                               _C.KV_PAGE_TOKENS, self.pages.n_pages * _C.KV_PAGE_TOKENS)
 
-    def check_prefix(self, slots: list, cols: int) -> None:
-        """Refuses (before any state is touched) an admission of `slots` whose first `cols` columns the pool cannot cover, counting
-        the pages the slots give back (a page still shared with a slot outside `slots` is not given back)."""
+    def check_prefix(self, slots: list, cols: int, prompt_cols: int = 0) -> None:
+        """Refuses (before any state is touched) an admission of `slots` whose first `cols` columns the pool cannot cover, or (with
+        cross-attention prompts) whose prompts of `prompt_cols` tokens the prompt pool cannot cover, counting the pages the slots give
+        back (a page still shared with a slot outside `slots` is not given back)."""
         need = len(slots) * self.pages.pages_for(cols)
         have = self.kv_pages_free + self.pages.freed_by(slots)
         if need > have:
             raise ValueError(f"admitting {len(slots)} prefixes of {cols} tokens needs {need} K/V pages, {have} are free: release "
                              "slots or open the cache with a larger kv_pool_tokens")
+        if self.Lp_cap:
+            need = len(slots) * self.prompt_pages.pages_for(prompt_cols)
+            have = self.prompt_pages_free + self.prompt_pages.freed_by(slots)
+            if need > have:
+                raise ValueError(f"admitting {len(slots)} prompts of {prompt_cols} tokens needs {need} prompt pages, {have} are free: "
+                                 "release slots or open the cache with a larger prompt_pool_tokens")
 
-    def free_slots(self, slots: list, prefix_cols: int = 0) -> None:
-        """Return the pages of `slots` (released or re-admitted) and give each `prefix_cols` columns of new ones (checked by
-        check_prefix).  Asynchronous, no host synchronisation."""
+    def free_slots(self, slots: list, prefix_cols: int = 0, prompt_cols: int = 0) -> None:
+        """Return the pages of `slots` (released or re-admitted), history and prompt, and give each `prefix_cols` columns of new
+        history pages and `prompt_cols` columns of new prompt pages (checked by check_prefix), the rows of the last prompt page past
+        `prompt_cols` zeroed.  Asynchronous, no host synchronisation."""
         upd = []
         for b in slots:
             upd += self.pages.release(b)
         for b in slots:
             upd += self.pages.reserve(b, prefix_cols)
         self._push_pages(upd)
+        if self.Lp_cap:
+            upd = []
+            for b in slots:
+                upd += self.prompt_pages.release(b)
+            for b in slots:
+                upd += self.prompt_pages.reserve(b, prompt_cols)
+            self._push_pages(upd, self.prompt_page_table)
+            if prompt_cols % _C.KV_PAGE_TOKENS:
+                self._zero_prompt_pages([self.prompt_pages.owned[b][-1] for b in slots])
+
+    def _zero_prompt_pages(self, pages: list) -> None:
+        """Copy the zero page over `pages` in every layer's prompt pool (one launch).  The attention kernels read whole pages, so the
+        rows of a prompt's last page past its length must hold no earlier tenant's values: a NaN there would reach the output as
+        0 * NaN."""
+        if not pages:
+            return
+        rows = self.device_ints([0] * len(pages) + [pg * _C.KV_PAGE_TOKENS for pg in pages]).view(2, len(pages))
+        _C.Context.get(self.page_table.device).kv_copy_blocks(self.copy_bufs("prompt"), self.prompt_kv_hi[0].stride(0) * 2, rows[0], rows[1],
+                                                              _C.KV_PAGE_TOKENS, self.prompt_pages.n_pages * _C.KV_PAGE_TOKENS)
 
     def check_fork(self, src, dst) -> tuple:
         """Everything that can refuse a fork, before any state is touched: -> (src, dst) as lists of ints."""
@@ -345,8 +405,9 @@ class SlotDecodeCache:
 
     def fork(self, src: list, dst: list) -> None:
         """Slot dst[i] takes a copy of slot src[i]'s episode (after check_fork): its pages by reference (the pages of the columns
-        [0, len) the source has written; no page is taken), its per-slot state, fed-back action, history mask, prompt mask and
-        prompt K/V rows.  A live destination lets go of its pages first.  Asynchronous, no host synchronisation."""
+        [0, len) the source has written, and all its prompt pages; no page is taken and no K/V row is copied), its per-slot state,
+        fed-back action, history mask, prompt mask and prompt length.  A live destination lets go of its pages first.  Asynchronous,
+        no host synchronisation."""
         if not dst:
             return
         upd = []
@@ -360,24 +421,28 @@ class SlotDecodeCache:
         si, di = idx[:n], idx[n:]
         rows = [self.len, self.n_valid, self.has_action, self.active, self.action_token, self.mask]
         if self.Lp_cap:
-            rows.append(self.prompt_mask)
-            starts = idx * self.Lp_cap
-            _C.Context.get(self.page_table.device).kv_copy_blocks(self.copy_bufs("prompt"), self.prompt_kv[0].hi.stride(0) * 2, starts[:n],
-                                                                  starts[n:], self.Lp_cap, self.S * self.Lp_cap)
+            upd = []
+            for b in dst:
+                upd += self.prompt_pages.release(b)
+            for a, b in zip(src, dst):
+                upd += self.prompt_pages.fork(a, b, len(self.prompt_pages.owned[a]))
+            self._push_pages(upd, self.prompt_page_table)
+            rows += [self.prompt_mask, self.prompt_len]
         for t in rows:
             t.index_copy_(0, di, t.index_select(0, si))
         for a, b in zip(src, dst):
             self.len_host[b], self.has_action_host[b], self.active_host[b] = self.len_host[a], self.has_action_host[a], True
 
-    def _push_pages(self, upd: list) -> None:
-        """Page-table entries (flat index, page) -> the device table: one copy from pinned host memory and one scatter, both queued
-        on the current stream.  A later entry for the same index wins (a re-admitted slot's page 0 of its released row is given
-        again): the scatter gets each index once, since its order among duplicates is undefined."""
+    def _push_pages(self, upd: list, table: Optional[torch.Tensor] = None) -> None:
+        """Page-table entries (flat index, page) -> the device table (default: the history pool's `page_table`): one copy from pinned
+        host memory and one scatter, both queued on the current stream.  A later entry for the same index wins (a re-admitted slot's
+        page 0 of its released row is given again): the scatter gets each index once, since its order among duplicates is
+        undefined."""
         last = dict(upd)
         if not last:
             return
         d = self.device_ints(list(last) + list(last.values())).view(2, len(last))
-        self.page_table.view(-1).scatter_(0, d[0], d[1].to(torch.int32))
+        (self.page_table if table is None else table).view(-1).scatter_(0, d[0], d[1].to(torch.int32))
 
     def device_ints(self, values: list) -> torch.Tensor:
         """int64 [len(values)] on the cache's device, copied from pinned host memory without a host synchronisation."""
@@ -670,24 +735,29 @@ class XAttnGPT(nn.Module):
     def admit_prompts(self, cache: SlotDecodeCache, slots: list, prompt_tokens: torch.Tensor, prompt_mask_u8: torch.Tensor,
                       prompt_position_ids: torch.Tensor) -> None:
         """Projected prompt keys/values of every layer for the n new prompts only (prompt_tokens (Lp,n,E), mask / position ids (n,Lp)),
-        scattered into `slots` of the cache; their prompt masks are padded to Lp_cap with masked columns and their state is reset to
-        an empty history.  The caller has validated shapes, slots and the precision mode."""
+        written into ceil(Lp/64) fresh prompt pages of each of `slots` (the rows past Lp of the last page are zero); their prompt
+        masks are padded to Lp_cap with masked columns, their prompt length is Lp and their state is reset to an empty history.  The
+        caller has validated shapes, slots and the precision mode; a prompt pool that cannot cover the admission raises ValueError
+        before any state is touched."""
+        Lp, n, E = prompt_tokens.shape
+        cache.check_prefix(slots, 0, Lp)
         ctx = eng.ctx_for(prompt_tokens)
         p = eng.prec()
-        Lp, n, E = prompt_tokens.shape
         dev = prompt_tokens.device
         self._pos_guard.poll()
         err = self._pos_guard.device_flag(dev)  # a bad prompt position id is reported by the next step
         kv16 = self._prompt_operand(ctx, p, prompt_tokens.float(), prompt_position_ids, False, n, Lp, E, err)
-        cache.free_slots(slots)  # a re-admitted slot's history pages go back to the pool; its first step takes new ones
+        # the slots' history pages go back to the pool (their first step takes new ones); their prompt pages are replaced
+        cache.free_slots(slots, prompt_cols=Lp)
         idx = cache.device_ints(slots)
-        for W, dst in zip(self._packed(ctx, p), cache.prompt_kv):
+        sl = idx.to(torch.int32)
+        for W, khi, klo in zip(self._packed(ctx, p), cache.prompt_kv_hi, cache.prompt_kv_lo):
             kv = eng.gemm(ctx, kv16, W["wkv"], p, want16=True)[1]
-            for d_t, s_t in ((dst.hi, kv.hi), (dst.lo, kv.lo)):
-                if d_t is not None:
-                    d_t.view(cache.S, cache.Lp_cap, -1)[idx, :Lp] = s_t[: n * Lp].view(n, Lp, -1)
+            ctx.slot_kv_scatter_paged(kv.hi, kv.lo, kv.ld, 0, 2 * E, n, Lp, sl, khi, klo, 2 * E, cache.prompt_page_table,
+                                      cache.prompt_pages.n_pages)
         cache.prompt_mask.index_fill_(0, idx, 0)
         cache.prompt_mask[idx, :Lp] = prompt_mask_u8
+        cache.prompt_len.index_fill_(0, idx, Lp)
         for t, v in ((cache.len, 0), (cache.n_valid, 0), (cache.has_action, 0), (cache.active, 1)):
             t.index_fill_(0, idx, v)
         for b in slots:
@@ -757,7 +827,7 @@ class XAttnGPT(nn.Module):
         # x = tokens + positions_embed[ids] (fp32 residual stream); kv = prompt + xattn_positions_embed[ids] (operands only)
         x32 = torch.empty((M, E), dtype=torch.float32, device=dev)
         ctx.add_pos_embed(tok, sb, sl, oa_ids, self.positions_embed.weight.detach(), B, L, E, out_f32=x32, err_flag=err)
-        need_prompt = cache is None or cache.prompt_kv is None
+        need_prompt = cache is None or (not slots and cache.prompt_kv is None)
         kv16 = self._prompt_operand(ctx, p, prompt_tokens, prompt_position_ids, batch_first, B, Lp, E, err) if need_prompt else None
         self._pos_guard.after_launch()  # first call: synchronous check; later: asynchronous copy, reported by the next call
         if cache is None:
@@ -773,11 +843,16 @@ class XAttnGPT(nn.Module):
         for i, (blk, xa, W) in enumerate(zip(self.h, self.xattns, layers)):
             # ---------------- XAttention ----------------
             _, q16 = eng.gemm(ctx, qin16, W["wq"], p, want16=True)
-            kvp16 = cache.prompt_kv[i] if cache is not None else eng.gemm(ctx, kv16, W["wkv"], p, want16=True)[1]
+            if slots:  # each slot's prompt through its page table, prompt_len[b] keys
+                khi, klo, kld = cache.prompt_kv_hi[i], cache.prompt_kv_lo[i], 2 * E
+                paged = dict(kv_pages=cache.prompt_page_table, kv_pool_pages=cache.prompt_pages.n_pages, kv_len=cache.prompt_len)
+            else:
+                kvp16 = cache.prompt_kv[i] if cache is not None else eng.gemm(ctx, kv16, W["wkv"], p, want16=True)[1]
+                khi, klo, kld, paged = kvp16.hi, kvp16.lo, kvp16.ld, {}
             c16 = eng.Opnd(M, E, dev, p.split, f8=p.f8)
-            ctx.attention(q=(q16.hi, q16.lo, q16.ld, 0), k=(kvp16.hi, kvp16.lo, kvp16.ld, 0), v=(kvp16.hi, kvp16.lo, kvp16.ld, E),
-                          o=(c16.hi, c16.lo, c16.ld, 0), B=B, H=Hx, Lq=L, Lk=Lp, D=d_x, scale=1.0 / math.sqrt(d_x), causal=False,
-                          key_mask=pmask, dtype=p.dtype, o8=None if c16.lo8 is None else (c16.lo8, c16.hi8))
+            ctx.attention(q=(q16.hi, q16.lo, q16.ld, 0), k=(khi, klo, kld, 0), v=(khi, klo, kld, E), o=(c16.hi, c16.lo, c16.ld, 0), B=B,
+                          H=Hx, Lq=L, Lk=Lp, D=d_x, scale=1.0 / math.sqrt(d_x), causal=False, key_mask=pmask, dtype=p.dtype,
+                          o8=None if c16.lo8 is None else (c16.lo8, c16.hi8), **paged)
             part = eng.stats_buffer(ctx, M, W["wo"], dev)
             a32, a16 = eng.gemm(ctx, c16, W["wo"], p, residual=x32, want_f32=True, want16=True, out_f8=True, stats_out=part)
             st = eng.row_stats_of(ctx, part, M, E, xa.ln.eps)

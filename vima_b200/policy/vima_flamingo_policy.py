@@ -102,8 +102,9 @@ class VIMAFlamingoPolicy(VIMAGatoPolicy):
         return VIMAPolicy.forward_step(self, cache, obs_token, self._ones(obs_token), prev_action_token)
 
     def open_slots(self, n_slots: int, *, max_tokens: Optional[int] = None, max_prompt_tokens: int = 256,
-                   kv_pool_tokens: Optional[int] = None):
-        return VIMAPolicy.open_slots(self, n_slots, max_tokens=max_tokens, max_prompt_tokens=max_prompt_tokens, kv_pool_tokens=kv_pool_tokens)
+                   kv_pool_tokens: Optional[int] = None, prompt_pool_tokens: Optional[int] = None):
+        return VIMAPolicy.open_slots(self, n_slots, max_tokens=max_tokens, max_prompt_tokens=max_prompt_tokens, kv_pool_tokens=kv_pool_tokens,
+                                     prompt_pool_tokens=prompt_pool_tokens)
 
     def admit(self, cache, slots, prompt_token: torch.Tensor, prompt_token_mask: torch.Tensor) -> None:
         eng.ctx_for(prompt_token)

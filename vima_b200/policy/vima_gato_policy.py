@@ -187,7 +187,7 @@ class VIMAGatoPolicy(nn.Module):
         Prefills the n new [prompt | separator] sequences only, on the current stream."""
         ctx = eng.ctx_for(prompt_token)
         s = cache.slot_index(slots)
-        if cache.prompt_kv is not None:
+        if cache.Lp_cap:
             raise ValueError("admit: this SlotDecodeCache was opened for a cross-attention decoder")
         self._check_prompt(prompt_token, prompt_token_mask, len(s), cache.Lmax)
         cache.check_precision(eng.prec())

@@ -150,11 +150,14 @@ class VIMAPolicy(nn.Module):
     # Slot decode (DESIGN.md 7 (f)1): each row of the batch is a slot holding one episode at a time, so episodes start and finish
     # independently (a vectorised environment resets each of its environments on its own).
     def open_slots(self, n_slots: int, *, max_tokens: Optional[int] = None, max_prompt_tokens: int = 256,
-                   kv_pool_tokens: Optional[int] = None):
+                   kv_pool_tokens: Optional[int] = None, prompt_pool_tokens: Optional[int] = None):
         """Allocate a SlotDecodeCache of `n_slots` slots (all inactive) with room for `max_tokens` history tokens (default: the
         decoder's n_positions) and `max_prompt_tokens` prompt tokens per episode, in the current precision mode.  The slots' history
         K/V live in a shared pool of 64-token pages holding `kv_pool_tokens` tokens (default: n_slots * max_tokens, rounded up to
-        whole pages per slot, so every slot can reach max_tokens at once); a smaller pool refuses a step it cannot cover."""
+        whole pages per slot, so every slot can reach max_tokens at once); a smaller pool refuses a step it cannot cover.  Their
+        projected prompt K/V live in a second pool of 64-token pages holding `prompt_pool_tokens` tokens (default: n_slots *
+        max_prompt_tokens, rounded up the same way); a smaller pool refuses an admission it cannot cover, and forked slots share
+        their source's prompt pages."""
         dev = self.xattn_gpt.positions_embed.weight.device
         eng.ctx_for(self.xattn_gpt.positions_embed.weight)
         Lmax = self.xattn_gpt.n_positions if max_tokens is None else int(max_tokens)
@@ -167,7 +170,7 @@ class VIMAPolicy(nn.Module):
         p = eng.prec()
         return vnn.SlotDecodeCache(S=int(n_slots), Lmax=Lmax, Lp_cap=int(max_prompt_tokens), E=self.embed_dim, n_layer=self.xattn_gpt.n_layer,
                                    device=dev, split=p.split, precision=p.name, weights=eng.WeightState([self.xattn_gpt]),
-                                   kv_pool_tokens=kv_pool_tokens)
+                                   kv_pool_tokens=kv_pool_tokens, prompt_pool_tokens=prompt_pool_tokens)
 
     def admit(self, cache, slots, prompt_token: torch.Tensor, prompt_token_mask: torch.Tensor) -> None:
         """Start a new episode in each of `slots` (replacing whatever they held): prompt_token (Lp,n,E), prompt_token_mask (n,Lp),
