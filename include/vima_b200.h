@@ -305,6 +305,13 @@ int vima_slot_admit_prefix(vima_ctx*, const int32_t* slots, int n, const uint8_t
  * is skipped, never written.  Destination blocks must not overlap any block's source rows. */
 int vima_kv_copy_blocks(vima_ctx*, void* const* bufs, int n_buf, int64_t row_bytes, const int64_t* src_row0, const int64_t* dst_row0,
                         int n_blocks, int block_rows, int64_t buf_rows, void* stream);
+/* Swapped slot episodes (no reference counterpart): move block i of block_rows rows at row row0[i] of each of the n_buf buffers
+ * (bufs, row_bytes, buf_rows and the skipping rules as vima_kv_copy_blocks) to or from one packed DEVICE buffer laid out
+ * [block][buffer][block_rows][row_bytes], so consecutive blocks are one contiguous slice.  unpack = 0: buffers -> packed (pack);
+ * unpack = 1: packed -> buffers.  row0: DEVICE int64 [n_blocks]; packed 16-byte aligned.  A skipped block's packed rows are
+ * neither read nor written.  Unpacked blocks must not overlap each other. */
+int vima_kv_pack_blocks(vima_ctx*, void* const* bufs, int n_buf, int64_t row_bytes, const int64_t* row0, int n_blocks, int block_rows,
+                        int64_t buf_rows, void* packed, int unpack, void* stream);
 /* out[b,l,:] = tok[b*stride_b + l*stride_l + :] + table[ids[b,l]]  (xattn_gpt.py:103-105,110-114); out-of-range
  * ids set *err_flag (device int) to 1 -- the reference raises IndexError there. */
 int vima_add_pos_embed(vima_ctx*, const float* tok, int64_t stride_b, int64_t stride_l, const int64_t* ids, const float* table, int n_pos,

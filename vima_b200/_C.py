@@ -115,7 +115,7 @@ EXPORTS = [
     "vima_gather_prompt", "vima_patchify", "vima_vit_tokens", "vima_bbox_norm", "vima_fill_ee", "vima_max_u8",
     "vima_action_scale", "vima_action_postprocess", "vima_latent_attention", "vima_object_stats", "vima_crop_resize", "vima_head_select", "vima_gato_positions", "vima_pack_weight_f8", "vima_split_f8",
     "vima_slot_step_begin", "vima_slot_kv_append", "vima_slot_step_end", "vima_slot_kv_scatter", "vima_slot_admit_prefix",
-    "vima_slot_kv_append_paged", "vima_slot_kv_scatter_paged", "vima_kv_copy_blocks",
+    "vima_slot_kv_append_paged", "vima_slot_kv_scatter_paged", "vima_kv_copy_blocks", "vima_kv_pack_blocks",
     "vima_head_sample", "vima_sizeof_head_sample_desc",
 ]
 
@@ -410,6 +410,16 @@ class Context:
         self._ck(self.lib.vima_kv_copy_blocks(self.h, c_void_p(bufs.data_ptr()), int(bufs.numel()), c_i64(row_bytes),
                                               c_void_p(src_row0.data_ptr()), c_void_p(dst_row0.data_ptr()), int(src_row0.numel()),
                                               int(block_rows), c_i64(buf_rows), c_void_p(self._s())), "kv_copy_blocks")
+
+    def kv_pack_blocks(self, bufs, row_bytes, row0, block_rows, buf_rows, packed, unpack):
+        """Block i of block_rows rows at row row0[i] of every buffer whose base address bufs (int64 [n_buf], device) lists <-> packed
+        [block][buffer][block_rows][row_bytes] (a device tensor); unpack=False packs, True unpacks.  row0 int64 [n_blocks] (device).
+        Blocks starting outside [0, buf_rows - block_rows] are skipped."""
+        assert bufs.dtype == torch.int64 and row0.dtype == torch.int64 and row0.is_contiguous() and packed.is_contiguous()
+        assert packed.numel() * packed.element_size() >= row0.numel() * bufs.numel() * block_rows * row_bytes
+        self._ck(self.lib.vima_kv_pack_blocks(self.h, c_void_p(bufs.data_ptr()), int(bufs.numel()), c_i64(row_bytes), c_void_p(row0.data_ptr()),
+                                              int(row0.numel()), int(block_rows), c_i64(buf_rows), c_void_p(packed.data_ptr()), int(bool(unpack)),
+                                              c_void_p(self._s())), "kv_pack_blocks")
 
     def add_pos_embed(self, tok, stride_b, stride_l, ids, table, B, L, E, *, out_f32=None, hi=None, lo=None, dtype=DT_F16, err_flag=None):
         self._ck(self.lib.vima_add_pos_embed(self.h, c_void_p(tok.data_ptr()), c_i64(stride_b), c_i64(stride_l), c_void_p(ids.data_ptr()),

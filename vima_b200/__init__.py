@@ -5,9 +5,10 @@ import torch
 
 from .engine import get_precision, refresh_weights, set_precision
 from .nn.action import ActionSampler
+from .nn.xattn_gpt import SwappedEpisode
 from .policy import VIMAFlamingoPolicy, VIMAGatoPolicy, VIMAGPTPolicy, VIMAPolicy
 
-__all__ = ["VIMAPolicy", "VIMAGatoPolicy", "VIMAGPTPolicy", "VIMAFlamingoPolicy", "create_policy_from_ckpt", "set_precision", "get_precision", "refresh_weights", "ActionSampler"]
+__all__ = ["VIMAPolicy", "VIMAGatoPolicy", "VIMAGPTPolicy", "VIMAFlamingoPolicy", "create_policy_from_ckpt", "set_precision", "get_precision", "refresh_weights", "ActionSampler", "SwappedEpisode"]
 
 
 def create_policy_from_ckpt(ckpt_path, device):

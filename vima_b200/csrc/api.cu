@@ -591,6 +591,19 @@ int vima_kv_copy_blocks(vima_ctx* c, void* const* bufs, int n_buf, int64_t row_b
            "kv_copy_blocks");
 }
 
+int vima_kv_pack_blocks(vima_ctx* c, void* const* bufs, int n_buf, int64_t row_bytes, const int64_t* row0, int n_blocks, int block_rows,
+                        int64_t buf_rows, void* packed, int unpack, void* stream) {
+  CHECK_CTX(c);
+  if (!bufs || !row0 || !packed) return fail(c, VIMA_E_INVALID, "kv_pack_blocks: null pointer");
+  if (((uintptr_t)bufs & 7) || ((uintptr_t)row0 & 7) || ((uintptr_t)packed & 15) || n_buf < 1 || n_buf > 65535 || row_bytes < 16 ||
+      (row_bytes & 15) || block_rows < 1 || n_blocks < 0 || buf_rows < 0 || (unpack != 0 && unpack != 1))
+    return fail(c, VIMA_E_INVALID, "kv_pack_blocks: 1 <= n_buf <= 65535, row_bytes a positive multiple of 16, block_rows >= 1, "
+                                   "n_blocks >= 0, buf_rows >= 0, unpack 0 or 1, 8-byte aligned device arrays, 16-byte aligned packed");
+  LAUNCHED(c, launch_kv_pack_blocks(bufs, n_buf, (long long)row_bytes, (const long long*)row0, n_blocks, block_rows, (long long)buf_rows,
+                                    packed, unpack, (cudaStream_t)stream),
+           "kv_pack_blocks");
+}
+
 int vima_add_pos_embed(vima_ctx* c, const float* tok, int64_t stride_b, int64_t stride_l, const int64_t* ids, const float* table, int n_pos, int B,
                        int L, int E, float* out_f32, void* hi, void* lo, int ld16, int dtype, int* err_flag, void* stream) {
   CHECK_CTX(c);

@@ -210,5 +210,9 @@ cudaError_t launch_slot_admit_prefix(const int* slots, int n, const unsigned cha
 // rows of row_bytes (a multiple of 16); blocks with a start outside [0, buf_rows - block_rows] are skipped.
 cudaError_t launch_kv_copy_blocks(void* const* bufs, int n_buf, long long row_bytes, const long long* src_row0, const long long* dst_row0,
                                   int n_blocks, int block_rows, long long buf_rows, cudaStream_t s);
+// Block i of rows [row0[i], +block_rows) of each buffer z <-> packed[i][z] ([block][buffer][block_rows][row_bytes]); unpack = 0 packs
+// (buffers -> packed), 1 unpacks.  Blocks with a start outside [0, buf_rows - block_rows] are skipped.
+cudaError_t launch_kv_pack_blocks(void* const* bufs, int n_buf, long long row_bytes, const long long* row0, int n_blocks, int block_rows,
+                                  long long buf_rows, void* packed, int unpack, cudaStream_t s);
 
 }  // namespace vima

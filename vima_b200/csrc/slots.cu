@@ -224,4 +224,38 @@ cudaError_t launch_kv_copy_blocks(void* const* bufs, int n_buf, long long row_by
   return cudaGetLastError();
 }
 
+// Block moves between the buffers and one packed buffer (swapped slot episodes).  Grid (row chunk, block, buffer): block i of buffer
+// z, rows [row0[i], +block_rows), <-> packed[i][z] of the layout [block][buffer][block_rows][row_bytes], 16 bytes per thread and
+// trip; `unpack` picks the direction (0: buffers -> packed).  A block whose start lies outside [0, buf_rows - block_rows], or a
+// buffer whose base is null or not 16-byte aligned, is skipped (its packed rows are neither read nor written).
+__global__ void __launch_bounds__(256) kv_pack_blocks_kernel(void* const* __restrict__ bufs, long long row16,
+                                                             const long long* __restrict__ row0, int n_blocks, int block_rows,
+                                                             long long buf_rows, uint4* __restrict__ packed, int unpack) {
+  uint4* buf = reinterpret_cast<uint4*>(bufs[blockIdx.z]);
+  if (buf == nullptr || (reinterpret_cast<uintptr_t>(buf) & 15)) return;
+  const long long n16 = (long long)block_rows * row16, last = buf_rows - block_rows;
+  for (int i = blockIdx.y; i < n_blocks; i += gridDim.y) {
+    const long long r = __ldg(row0 + i);
+    if (r < 0 || r > last) continue;
+    uint4* rows = buf + r * row16;
+    uint4* pk = packed + ((long long)i * gridDim.z + blockIdx.z) * n16;
+    for (long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x; j < n16; j += (long long)gridDim.x * blockDim.x) {
+      if (unpack)
+        rows[j] = pk[j];
+      else
+        pk[j] = rows[j];
+    }
+  }
+}
+
+cudaError_t launch_kv_pack_blocks(void* const* bufs, int n_buf, long long row_bytes, const long long* row0, int n_blocks, int block_rows,
+                                  long long buf_rows, void* packed, int unpack, cudaStream_t s) {
+  if (n_blocks == 0) return cudaSuccess;
+  const long long n16 = (long long)block_rows * (row_bytes / 16);
+  const dim3 grid((unsigned)min((n16 + 255) / 256, 1024ll), (unsigned)min(n_blocks, 65535), (unsigned)n_buf);
+  kv_pack_blocks_kernel<<<grid, 256, 0, s>>>(bufs, row_bytes / 16, row0, n_blocks, block_rows, buf_rows, reinterpret_cast<uint4*>(packed),
+                                             unpack);
+  return cudaGetLastError();
+}
+
 }  // namespace vima

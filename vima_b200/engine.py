@@ -316,6 +316,10 @@ class WeightState:
             return "the weights changed (a parameter was replaced, written in place, or refresh_weights was called)"
         return None
 
+    def matches(self, other: "WeightState") -> bool:
+        """Both were taken of the same parameters and packed-weight caches at the same versions, and neither has changed since."""
+        return self._fp == other._fp and self.changed() is None and other.changed() is None
+
 
 class _Recorder:
     def __init__(self):

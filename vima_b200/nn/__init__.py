@@ -14,4 +14,4 @@ from .obj_encoder import (GatoMultiViewRGBEncoder, GatoViTEncoder, MultiViewRGBE
                           VisionTransformer)
 from .perceiver import ObjectsPerceiverEncoder
 from .t5_encoder import T5PromptEncoder, WordEmbedding
-from .xattn_gpt import HFGPT, DecodeCache, SlotDecodeCache, XAttnGPT
+from .xattn_gpt import HFGPT, DecodeCache, SlotDecodeCache, SwappedEpisode, XAttnGPT

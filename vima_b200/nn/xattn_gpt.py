@@ -193,6 +193,27 @@ class KVPagePool:
         self.free, self.owned, self.refs = list(st[0]), [list(o) for o in st[1]], list(st[2])
 
 
+class SwappedEpisode:
+    """One slot episode parked in pinned host memory by `swap_out` (DESIGN.md 7 (f)1), to be written back by `swap_in` into a slot
+    of any cache of the same policy, precision mode and shapes, as often as wanted.  `kv` holds its history pages (the `kv_pages`
+    whole pages of its columns [0, len)) and `prompt` its `prompt_pages` prompt pages (cross-attention policies), both packed
+    [page][buffer][64 rows][row bytes] over every layer's hi and lo pool; `state` is its record of the per-slot device state (len,
+    n_valid, has_action, fed-back action token, history mask, prompt length and mask); `len_host` / `has_action_host` are the
+    host mirrors.  The three are views of the pinned buffer of one swap_out call."""
+
+    def __init__(self, *, kv, prompt, state, kv_pages: int, prompt_pages: int, len_host: int, has_action_host: bool, key: tuple, weights):
+        self.kv, self.prompt, self.state = kv, prompt, state
+        self.kv_pages, self.prompt_pages = kv_pages, prompt_pages
+        self.len_host, self.has_action_host = len_host, has_action_host
+        self.key = key  # SlotDecodeCache.swap_key() of the source cache: swap_in refuses a cache of another
+        self.weights = weights  # the source cache's engine.WeightState: its K/V rows were computed with these weights
+
+    @property
+    def nbytes(self) -> int:
+        """Pinned host bytes of the episode (K/V pages, prompt pages and state)."""
+        return self.kv.numel() + self.prompt.numel() + self.state.numel()
+
+
 class SlotDecodeCache:
     """K/V cache of `S` slots, each holding one episode at its own history length (DESIGN.md 4 and 7 (f)1).
 
@@ -432,6 +453,182 @@ class SlotDecodeCache:
             t.index_copy_(0, di, t.index_select(0, si))
         for a, b in zip(src, dst):
             self.len_host[b], self.has_action_host[b], self.active_host[b] = self.len_host[a], self.has_action_host[a], True
+
+    # ---- swapped episodes: a slot's episode to pinned host memory and back (DESIGN.md 7 (f)1)
+    def swap_key(self) -> tuple:
+        """What a swapped episode must share with the cache it is swapped into: (precision mode, Lmax, Lp_cap, E, layers, split)."""
+        return (self.precision, self.Lmax, self.Lp_cap, self.E, len(self.kv_hi), self.kv_lo[0] is not None)
+
+    def kv_pages_freed_by(self, slots) -> int:
+        """History pages that swapping out or releasing `slots` would return to the free list (a page that a slot outside `slots`
+        still holds, a fork's, stays)."""
+        return self.pages.freed_by(self.slot_index(slots))
+
+    def check_swap_out(self, slots) -> list:
+        """Everything that can refuse a swap-out, before any state is touched: -> slots as a list of ints."""
+        s = self.slot_index(slots)
+        bad = [b for b in s if not self.active_host[b]]
+        if bad:
+            raise ValueError(f"swap_out: slots {bad} are not active")
+        return s
+
+    def swap_out(self, slots: list) -> list:
+        """The episodes of `slots` (after check_swap_out) -> SwappedEpisode each: their history pages of columns [0, len), their prompt
+        pages and state rows, packed on the device and copied to one pinned host buffer; then the slots are released (a page still
+        shared with a fork stays with the fork).  Asynchronous, no host synchronisation: the host buffer is complete once the work
+        queued on the current stream so far has run."""
+        if not slots:
+            return []
+        kv = [self.pages.owned[b][:self.pages.pages_for(self.len_host[b])] for b in slots]
+        pr = [list(self.prompt_pages.owned[b]) if self.Lp_cap else [] for b in slots]
+        views = self._swap_out_data(slots, kv, pr)
+        key = self.swap_key()
+        eps = [SwappedEpisode(kv=k, prompt=p, state=st, kv_pages=len(kv[i]), prompt_pages=len(pr[i]), len_host=self.len_host[b],
+                              has_action_host=self.has_action_host[b], key=key, weights=self.weights)
+               for i, (b, (k, p, st)) in enumerate(zip(slots, views))]
+        self.active.index_fill_(0, self.device_ints(slots), 0)  # what release does
+        self.free_slots(slots)
+        for b in slots:
+            self.active_host[b] = False
+        return eps
+
+    def check_swap_in(self, slots, episodes) -> tuple:
+        """Everything that can refuse a swap-in, before any state is touched: -> (slots, episodes) as lists.  The pools must cover
+        the episodes' pages, counting the pages the destinations give back (as check_prefix does)."""
+        s = self.slot_index(slots)
+        eps = list(episodes)
+        if len(eps) != len(s):
+            raise ValueError(f"swap_in: {len(eps)} episodes for {len(s)} slots")
+        key = self.swap_key()
+        for i, ep in enumerate(eps):
+            if not isinstance(ep, SwappedEpisode):
+                raise ValueError(f"swap_in: episode {i} is a {type(ep).__name__}, not a SwappedEpisode")
+            if ep.key != key:
+                raise ValueError(f"swap_in: episode {i} comes from a cache of (precision, max_tokens, max_prompt_tokens, E, layers, split) = "
+                                 f"{ep.key}; this cache is {key}")
+            if (ep.weights is None) != (self.weights is None) or (ep.weights is not None and not ep.weights.matches(self.weights)):
+                raise ValueError(f"swap_in: episode {i}'s K/V rows belong to other weights (another policy's, or weights changed since "
+                                 "the swap-out or since this cache was opened)")
+        need, have = sum(ep.kv_pages for ep in eps), self.kv_pages_free + self.pages.freed_by(s)
+        if need > have:
+            raise ValueError(f"swap_in: {len(eps)} episodes need {need} K/V pages, {have} are free: release or swap out slots, or open "
+                             "the cache with a larger kv_pool_tokens")
+        if self.Lp_cap:
+            need, have = sum(ep.prompt_pages for ep in eps), self.prompt_pages_free + self.prompt_pages.freed_by(s)
+            if need > have:
+                raise ValueError(f"swap_in: {len(eps)} episodes need {need} prompt pages, {have} are free: release or swap out slots, "
+                                 "or open the cache with a larger prompt_pool_tokens")
+        return s, eps
+
+    def swap_in(self, slots: list, episodes: list) -> None:
+        """Slot slots[i] resumes episodes[i] (after check_swap_in) exactly where it was swapped out: the destination lets go of its
+        pages (a live one is replaced), takes private pages for the episode's history and prompt pages, and gets their rows, its state
+        rows and host mirrors back.  The episodes stay usable.  Asynchronous, no host synchronisation."""
+        if not slots:
+            return
+        upd, kv = [], []
+        for b in slots:
+            upd += self.pages.release(b)
+        for b, ep in zip(slots, episodes):
+            upd += self.pages.reserve(b, ep.kv_pages * _C.KV_PAGE_TOKENS)
+            kv.append(list(self.pages.owned[b]))
+        self._push_pages(upd)
+        pr = [[] for _ in slots]
+        if self.Lp_cap:
+            upd = []
+            for b in slots:
+                upd += self.prompt_pages.release(b)
+            for i, (b, ep) in enumerate(zip(slots, episodes)):
+                upd += self.prompt_pages.reserve(b, ep.prompt_pages * _C.KV_PAGE_TOKENS)
+                pr[i] = list(self.prompt_pages.owned[b])
+            self._push_pages(upd, self.prompt_page_table)
+        self._swap_in_data(slots, episodes, kv, pr)
+        for b, ep in zip(slots, episodes):
+            self.len_host[b], self.has_action_host[b], self.active_host[b] = ep.len_host, ep.has_action_host, True
+
+    def _state_layout(self) -> tuple:
+        """([(device state tensor [S, ...], byte offset, bytes)], record bytes): one slot's state rows in a swapped episode's record,
+        4-byte fields first; the record size is a multiple of 16."""
+        rows = [self.len, self.n_valid, self.has_action] + ([self.prompt_len] if self.Lp_cap else [])
+        rows += [self.action_token, self.mask] + ([self.prompt_mask] if self.Lp_cap else [])
+        out, off = [], 0
+        for t in rows:
+            nb = t[0].numel() * t.element_size()
+            out.append((t, off, nb))
+            off += nb
+        return out, -(-off // 16) * 16
+
+    @staticmethod
+    def _field(rec: torch.Tensor, t: torch.Tensor, off: int, nb: int) -> torch.Tensor:
+        """Field (t, off, nb) of the records rec uint8 [n, record bytes], as a [n, ...] view of t's dtype."""
+        return rec[:, off:off + nb].view(t.dtype).view((rec.shape[0],) + tuple(t.shape[1:]))
+
+    def _page_bytes(self, which: str) -> int:
+        """Packed bytes of one page of the "pool" (history) or "prompt" pool across every layer's hi and lo buffers."""
+        ts = self.kv_hi + self.kv_lo if which == "pool" else self.prompt_kv_hi + self.prompt_kv_lo
+        ts = [t for t in ts if t is not None]
+        return len(ts) * _C.KV_PAGE_TOKENS * ts[0].stride(0) * ts[0].element_size()
+
+    def _pack_pages(self, which: str, pages: list, packed: torch.Tensor, unpack: bool) -> None:
+        """`pages` of the "pool" or "prompt" pool <-> packed (device uint8), one vima_kv_pack_blocks launch."""
+        if not pages:
+            return
+        t0, n_pages = (self.kv_hi[0], self.pages.n_pages) if which == "pool" else (self.prompt_kv_hi[0], self.prompt_pages.n_pages)
+        rows = self.device_ints([pg * _C.KV_PAGE_TOKENS for pg in pages])
+        _C.Context.get(self.page_table.device).kv_pack_blocks(self.copy_bufs(which), t0.stride(0) * t0.element_size(), rows,
+                                                              _C.KV_PAGE_TOKENS, n_pages * _C.KV_PAGE_TOKENS, packed, unpack)
+
+    def _swap_out_data(self, slots: list, kv: list, prompt: list) -> list:
+        """Device side of swap_out: the history pages kv[i] and prompt pages prompt[i] of slot slots[i] (one pack launch per pool) and
+        its state rows (index_select) into one device staging buffer, copied to one pinned host buffer -> [(kv, prompt, state)] views
+        of it per episode."""
+        dev = self.page_table.device
+        kb, pb = self._page_bytes("pool"), (self._page_bytes("prompt") if self.Lp_cap else 0)
+        lay, rec = self._state_layout()
+        n = len(slots)
+        k_end = sum(map(len, kv)) * kb
+        p_end = k_end + sum(map(len, prompt)) * pb
+        stage = torch.empty(p_end + n * rec, dtype=torch.uint8, device=dev)
+        self._pack_pages("pool", [pg for ps in kv for pg in ps], stage[:k_end], False)
+        if self.Lp_cap:
+            self._pack_pages("prompt", [pg for ps in prompt for pg in ps], stage[k_end:p_end], False)
+        st = stage[p_end:].view(n, rec)
+        idx = self.device_ints(slots)
+        for t, off, nb in lay:
+            self._field(st, t, off, nb).copy_(t.index_select(0, idx))
+        host = torch.empty(stage.numel(), dtype=torch.uint8, pin_memory=True)
+        host.copy_(stage, non_blocking=True)
+        out, ko, po = [], 0, k_end
+        for i in range(n):
+            k, p = len(kv[i]) * kb, len(prompt[i]) * pb
+            out.append((host[ko:ko + k], host[po:po + p], host[p_end + i * rec:p_end + (i + 1) * rec]))
+            ko, po = ko + k, po + p
+        return out
+
+    def _swap_in_data(self, slots: list, episodes: list, kv: list, prompt: list) -> None:
+        """Device side of swap_in: the episodes copied from pinned host memory into one device staging buffer, their history pages
+        unpacked into kv[i] and prompt pages into prompt[i] (one unpack launch per pool), their state rows index_copy_'d into
+        slots[i], which become active."""
+        dev = self.page_table.device
+        lay, rec = self._state_layout()
+        n = len(slots)
+        k_end = sum(ep.kv.numel() for ep in episodes)
+        p_end = k_end + sum(ep.prompt.numel() for ep in episodes)
+        stage = torch.empty(p_end + n * rec, dtype=torch.uint8, device=dev)
+        ko, po = 0, k_end
+        for i, ep in enumerate(episodes):
+            for src, o in ((ep.kv, ko), (ep.prompt, po), (ep.state, p_end + i * rec)):
+                if src.numel():
+                    stage[o:o + src.numel()].copy_(src, non_blocking=True)
+            ko, po = ko + ep.kv.numel(), po + ep.prompt.numel()
+        self._pack_pages("pool", [pg for ps in kv for pg in ps], stage[:k_end], True)
+        if self.Lp_cap:
+            self._pack_pages("prompt", [pg for ps in prompt for pg in ps], stage[k_end:p_end], True)
+        st = stage[p_end:].view(n, rec)
+        idx = self.device_ints(slots)
+        for t, off, nb in lay:
+            t.index_copy_(0, idx, self._field(st, t, off, nb).contiguous())
+        self.active.index_fill_(0, idx, 1)
 
     def _push_pages(self, upd: list, table: Optional[torch.Tensor] = None) -> None:
         """Page-table entries (flat index, page) -> the device table (default: the history pool's `page_table`): one copy from pinned

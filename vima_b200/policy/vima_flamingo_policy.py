@@ -112,6 +112,8 @@ class VIMAFlamingoPolicy(VIMAGatoPolicy):
 
     release = VIMAPolicy.release
     fork_slots = VIMAPolicy.fork_slots
+    swap_out = VIMAPolicy.swap_out
+    swap_in = VIMAPolicy.swap_in
 
     def step_slots(self, cache, obs_token: torch.Tensor, action_token: Optional[torch.Tensor]) -> torch.Tensor:
         """obs_token (1,S,Q,E), action_token (1,S,E) | None -> (1,S,E), as VIMAPolicy.step_slots with every obs token valid."""

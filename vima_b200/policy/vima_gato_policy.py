@@ -198,6 +198,8 @@ class VIMAGatoPolicy(nn.Module):
 
     release = VIMAPolicy.release
     fork_slots = VIMAPolicy.fork_slots
+    swap_out = VIMAPolicy.swap_out
+    swap_in = VIMAPolicy.swap_in
     refresh_weights = VIMAPolicy.refresh_weights
 
     def step_slots(self, cache, obs_token: torch.Tensor, action_token: Optional[torch.Tensor]) -> torch.Tensor:

@@ -211,6 +211,30 @@ class VIMAPolicy(nn.Module):
         cache.check_precision(eng.prec())
         cache.fork(s, d)
 
+    def swap_out(self, cache, slots) -> list:
+        """Park the episodes of `slots` in pinned host memory and release the slots: -> one vima_b200.SwappedEpisode per slot, holding
+        the episode's history K/V pages, prompt K/V pages, fed-back action and state, so `swap_in` can resume it later exactly where
+        it stands.  The slots' pages go back to the pools (a page still shared with a fork stays with the fork), so a driver whose
+        overcommitted pool cannot cover the next step can preempt episodes instead of dropping them; `cache.kv_pages_freed_by(slots)`
+        says how many pages a choice of slots frees.  Refuses (ValueError, nothing touched) an inactive, out-of-range or repeated
+        slot and a cache of another precision mode or of changed weights.  Queued on the current stream, no host synchronisation:
+        the episodes' host buffers are filled once the stream reaches the copies."""
+        s = cache.check_swap_out(slots)
+        cache.check_precision(eng.prec())
+        return cache.swap_out(s)
+
+    def swap_in(self, cache, slots, episodes) -> None:
+        """Resume `episodes` (SwappedEpisode, from `swap_out` of this cache or of another cache of the same policy, precision mode,
+        max_tokens and max_prompt_tokens) in `slots`: slot slots[i] continues episodes[i] bit for bit as if it had never left.  A live
+        destination's episode is replaced; an episode can be swapped in again, into several slots or caches (each takes private
+        pages).  Refuses (ValueError, nothing touched) out-of-range or repeated slots, a count that does not match, an episode of
+        another precision mode, shape or policy or of weights changed since its swap-out, a cache of changed weights, and pools that
+        cannot cover the episodes' pages (counting those the destinations give back).  Queued on the current stream, no host
+        synchronisation."""
+        s, eps = cache.check_swap_in(slots, episodes)
+        cache.check_precision(eng.prec())
+        cache.swap_in(s, eps)
+
     def step_slots(self, cache, obs_token: torch.Tensor, obs_mask: torch.Tensor, action_token: Optional[torch.Tensor]) -> torch.Tensor:
         """One environment step of every slot: obs_token (1,S,Q,E), obs_mask (1,S,Q), action_token (1,S,E) (the previous action of
         each slot; ignored for slots at their first step; None = all zeros) -> predicted action token (1,S,E).  For an active slot
