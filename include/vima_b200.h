@@ -297,6 +297,23 @@ int vima_slot_kv_scatter_paged(vima_ctx*, const void* qkv_hi, const void* qkv_lo
  * len[b] = Lp+1, n_valid[b] = sum(prompt_mask[j] != 0) + 1, has_action[b] = 0, active[b] = 1.  Lp + 1 <= Lmax. */
 int vima_slot_admit_prefix(vima_ctx*, const int32_t* slots, int n, const uint8_t* prompt_mask, int Lp, int Lmax, uint8_t* slot_mask,
                            int32_t* len, int32_t* n_valid, int32_t* has_action, int32_t* active, void* stream);
+/* Slot episodes admitted mid-way from a recorded history (no reference counterpart: it re-runs the whole history every step).  Episode
+ * j has completed k_j = steps[j] environment steps (DEVICE int32 [n], clamped to [0, T]); its history columns are forward's
+ * [o_0 (Q tokens), a_0, o_1, ..., a_{k-2}, o_{k-1}]: k_j(Q+1) - 1 of them, 0 for k_j = 0.  Rows t >= k_j of obs / obs_mask / action
+ * are never read.
+ * slot_assemble_history: obs fp32 (T, n, Q, E), obs_mask uint8 (T, n, Q) (NULL = every obs token valid), action fp32 (T, n, E) ->
+ * rows [P, L) of tokens fp32 (L, n, E) and columns [P, L) of mask uint8 [n, L] / pos int64 [n, L]: history column c of episode j
+ * goes to column P + c; pos = (valid columns of mask[j, 0:P), written by the caller) + cumsum(history mask) - 1.  Columns past
+ * the history get a zero token, mask 0 and position id 0.  E % 4 == 0; obs, action, tokens 16-byte aligned.
+ * slot_admit_history: for each episode j, slot b = slots[j] (DEVICE int32 [n]; skipped outside [0, S) or when P + its history
+ * columns exceed L): slot_mask[b, c] = mask[j, c] for c < len, 0 for len <= c < Lmax, where len = P + history columns;
+ * len[b] = len, n_valid[b] = valid columns of mask[j, 0:len], has_action[b] = (k_j > 0), active[b] = 1, and for k_j > 0
+ * action_token[b] (fp32 [S, E]) = action[k_j - 1, j].  L <= Lmax. */
+int vima_slot_assemble_history(vima_ctx*, const float* obs, const uint8_t* obs_mask, const float* action, const int32_t* steps, int T, int n,
+                               int Q, int E, int P, int L, float* tokens, uint8_t* mask, int64_t* pos, void* stream);
+int vima_slot_admit_history(vima_ctx*, const int32_t* slots, const int32_t* steps, int n, int S, int T, int Q, int P, int L,
+                            const uint8_t* mask, const float* action, int E, int Lmax, uint8_t* slot_mask, int32_t* len, int32_t* n_valid,
+                            int32_t* has_action, int32_t* active, float* action_token, void* stream);
 /* Forked slots (no reference counterpart: it runs one episode per call): copy block i of block_rows rows from row src_row0[i] to row
  * dst_row0[i] in each of n_buf buffers of the same row width -- the copy on write of a shared K/V page (block_rows = 64, every
  * layer's hi and lo pool) and a fork's prompt K/V rows (block_rows = Lp_cap).  bufs: DEVICE array of n_buf base pointers, each a

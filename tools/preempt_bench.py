@@ -1,4 +1,4 @@
-"""Preemption by swapping on an overcommitted K/V pool: two drivers of the same episode schedule, alternated in one process.
+"""Preemption on an overcommitted K/V pool: three drivers of the same episode schedule, alternated in one process.
 
 The schedule is slot_decode_bench.py's: --episodes episodes of 1..--max-steps environment steps (seeded), --slots slots, cfg3 shapes
 by default (VIMA-200M, Q = 32 obs tokens, Lp = 256, f16f8); `--policy gato` runs cfg5 (VIMA-Gato-200M, prompt and separator in
@@ -10,11 +10,18 @@ schedule's peak page count, so it cannot hold every episode at its longest:
   swap      admit when the episode's prefix and first step fit; before each tick, while the step needs more pages than are free, swap out the
             most recently admitted active episode (policy.swap_out, to pinned host memory); swapped episodes are resumed
             (policy.swap_in), oldest first, before any new episode is admitted
+  recompute preempt as `swap` does but with policy.release alone, keeping each parked episode's record on the device (the bank
+            rows of its observations and the actions it took); parked episodes are resumed oldest first, before any new episode is
+            admitted, by policy.admit_history from that record (action tokens from forward_action_token of the recorded actions),
+            as many per call as fit
 
 Each run reports env-steps/s and episodes/s, ticks, preemptions, bytes swapped each way, the swap-out and swap-in rates (bytes over
 the CUDA-event time of the swap calls), the peak pinned host bytes held by parked episodes and torch.cuda.max_memory_allocated.
 An episode's k-th step takes the same inputs in both runs, so with --check the tool asserts that every episode's per-step actions
-in `swap` equal those in `reserve`.  Weights are random (timing only).  Prints the GPU's name and power limit beside the numbers,
+in `swap` equal those in `reserve`, and reports the number of episode steps whose actions in `recompute` differ from `reserve`
+(recomputed K/V match the stepped ones within the bars of forward_step, not bit for bit, so a near-tied greedy choice can flip).
+`recompute` also reports the CUDA-event time of its admit_history calls, the history rows they ran (episodes x padded length) and
+the peak device bytes of the parked records.  Weights are random (timing only).  Prints the GPU's name and power limit beside the numbers,
 one JSON line per run.
 """
 import argparse
@@ -45,8 +52,10 @@ def main():
     ap.add_argument("--precision", default="f16f8")
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--kv-pool-tokens", type=int, default=None, help="history pool in tokens (default: half the schedule's peak pages)")
-    ap.add_argument("--rounds", type=int, default=2, help="each round runs reserve then swap")
-    ap.add_argument("--check", action="store_true", help="assert that both drivers take the same actions in every episode")
+    ap.add_argument("--rounds", type=int, default=2, help="each round runs the drivers in turn")
+    ap.add_argument("--modes", default="reserve,swap,recompute", help="drivers of each round, in order")
+    ap.add_argument("--check", action="store_true", help="assert that swap takes the actions of reserve in every episode; count the "
+                                                         "episode steps where recompute does not")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("preempt_bench needs a CUDA device")
@@ -86,11 +95,35 @@ def main():
         idx = torch.tensor([e % P for e in eps], device="cuda")
         pol.admit(cache, slots, prompts[:, idx].contiguous(), pmask[idx].contiguous())
 
+    widths = {}  # action key -> head count, in sorted key order (the columns of act's result)
+
     def act(cache, rows):
         idx = torch.tensor(rows, device="cuda")
         obs = obs_bank[idx].unsqueeze(0)
         r = pol.act_slots(cache, obs, msk_bank[idx].unsqueeze(0)) if vima else pol.act_slots(cache, obs)
+        if not widths:
+            widths.update({k: r[0][k].shape[-1] for k in sorted(r[0])})
         return torch.cat([r[0][k][0] for k in sorted(r[0])], dim=1)
+
+    def resume(cache, slots, eps, done, recs):
+        """admit_history of parked episodes eps (done[e] steps each, recs[e] their action rows) into slots: one call."""
+        k = [done[e] for e in eps]
+        T = max(max(k), 1)
+        rows = torch.tensor([[(7 * e + t) % N if t < kk else 0 for e, kk in zip(eps, k)] for t in range(T)], device="cuda")
+        n_act = sum(widths.values())
+        zero = torch.zeros(n_act, dtype=torch.int64, device="cuda")
+        acts = torch.stack([torch.stack(recs.get(e, []) + [zero] * (T - len(recs.get(e, [])))) for e in eps], 1)  # (T, n, n_act)
+        d, c0 = {}, 0
+        for key, w in widths.items():
+            d[key] = acts[..., c0:c0 + w]
+            c0 += w
+        at = pol.forward_action_token(d)
+        idx = torch.tensor([e % P for e in eps], device="cuda")
+        pt, pm = prompts[:, idx].contiguous(), pmask[idx].contiguous()
+        if vima:
+            pol.admit_history(cache, slots, pt, pm, obs_bank[rows], msk_bank[rows], at, k)
+        else:
+            pol.admit_history(cache, slots, pt, pm, obs_bank[rows], at, k)
 
     def run(mode, record):
         """-> (ticks, stats); record[(episode, k)] = actions of the episode's k-th step (on the device) when record is a dict."""
@@ -98,10 +131,12 @@ def main():
         queue = list(range(len(lengths)))
         ep_of = [None] * S       # episode in each slot
         done = {}                # steps taken by each started episode
-        parked = []              # (episode, SwappedEpisode, swap call id), oldest episode first
+        parked = []              # (episode, SwappedEpisode, swap call id), oldest episode first; recompute: (episode, None, None)
         calls, live_pinned, peak_pinned = {}, 0, 0
-        ev_out, ev_in = [], []
+        ev_out, ev_in, ev_re = [], [], []
         out_bytes = in_bytes = preempt = ticks = 0
+        recs, rec_bytes, peak_rec, re_rows, re_eps = {}, 0, 0, 0, 0  # recompute: each started episode's action rows on the device
+        n_act = sum(widths.values()) * 8
         acts = []
         while queue or parked or any(e is not None for e in ep_of):
             free = [b for b in range(S) if ep_of[b] is None]
@@ -121,6 +156,29 @@ def main():
                     calls[cid][1] -= 1
                     if not calls[cid][1]:
                         live_pinned -= calls.pop(cid)[0]
+            if mode == "recompute":
+                group = []
+                room = cache.kv_pages_free - cache.kv_pages_needed(Q)
+                proom = cache.prompt_pages_free
+                while parked and free:
+                    e = parked[0][0]
+                    need = pages(prefix + (done[e] * (Q + 1) - 1 if done[e] else 0) + Q + 1)  # its history and its next step
+                    if need > room or (vima and pages(Lp) > proom):
+                        break
+                    parked.pop(0)
+                    group.append((free.pop(0), e))
+                    room -= need
+                    proom -= pages(Lp) if vima else 0
+                if group:
+                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    e0.record()
+                    resume(cache, [b for b, _ in group], [e for _, e in group], done, recs)
+                    e1.record()
+                    ev_re.append((e0, e1))
+                    re_rows += len(group) * max(prefix + (done[e] * (Q + 1) - 1 if done[e] else 0) for _, e in group)
+                    re_eps += len(group)
+                    for b, e in group:
+                        ep_of[b] = e
             take = []
             if mode == "reserve":
                 budget = cache.kv_pages_total - sum(worst for e in ep_of if e is not None)
@@ -136,6 +194,14 @@ def main():
                 admit(cache, [b for b, _ in take], [e for _, e in take])
                 for b, e in take:
                     ep_of[b], done[e] = e, 0
+            if mode == "recompute":
+                while cache.kv_pages_needed(Q) > cache.kv_pages_free:
+                    b = max((b for b in range(S) if ep_of[b] is not None), key=lambda b: ep_of[b])
+                    pol.release(cache, [b])
+                    preempt += 1
+                    parked.append((ep_of[b], None, None))
+                    parked.sort(key=lambda x: x[0])
+                    ep_of[b] = None
             if mode == "swap":
                 while cache.kv_pages_needed(Q) > cache.kv_pages_free:
                     b = max((b for b in range(S) if ep_of[b] is not None), key=lambda b: ep_of[b])
@@ -161,10 +227,16 @@ def main():
                 acts.append((out, [(b, ep_of[b], done[ep_of[b]]) for b in active]))
             ended = []
             for b in active:
+                if mode == "recompute":
+                    recs.setdefault(ep_of[b], []).append(out[b])
+                    rec_bytes += n_act
                 done[ep_of[b]] += 1
                 if done[ep_of[b]] == lengths[ep_of[b]]:
                     ended.append(b)
+                    if mode == "recompute":
+                        rec_bytes -= n_act * len(recs.pop(ep_of[b]))
                     ep_of[b] = None
+            peak_rec = max(peak_rec, rec_bytes)
             if ended:
                 pol.release(cache, ended)
         torch.cuda.synchronize()
@@ -177,7 +249,8 @@ def main():
                        "swap_out_GBps": round(out_bytes / ms(ev_out) / 1e6, 2) if ev_out else None,
                        "swap_in_GBps": round(in_bytes / ms(ev_in) / 1e6, 2) if ev_in else None,
                        "swap_out_ms_total": round(ms(ev_out), 2), "swap_in_ms_total": round(ms(ev_in), 2),
-                       "peak_pinned_host_bytes": peak_pinned}
+                       "peak_pinned_host_bytes": peak_pinned, "admit_history_ms_total": round(ms(ev_re), 2),
+                       "resumed_episodes": re_eps, "recomputed_rows": re_rows, "peak_record_device_bytes": peak_rec}
 
     with torch.no_grad():
         # warm-up: modules, weight packing, kernel attributes, one swap round trip
@@ -187,11 +260,13 @@ def main():
         for _ in range(2):
             act(c, [0] * S)
         pol.swap_in(c, [0], pol.swap_out(c, [0]))
+        pol.release(c, [0])
+        resume(c, [0], [0], {0: 2}, {0: [act(c, [0] * S)[0]] * 2})
         del c
         torch.cuda.synchronize()
         recs = {}
         for rnd in range(a.rounds):
-            for mode in ("reserve", "swap"):
+            for mode in a.modes.split(","):
                 rec = {} if (a.check and rnd == 0) else None
                 torch.cuda.synchronize()
                 torch.cuda.reset_peak_memory_stats()
@@ -205,11 +280,20 @@ def main():
                 if rec is not None:
                     recs[mode] = rec
         if a.check:
-            x, y = recs["reserve"], recs["swap"]
-            assert len(x) == total_steps and x.keys() == y.keys(), (len(x), len(y))
-            bad = [k for k in x if not torch.equal(x[k], y[k])]
-            assert not bad, f"{len(bad)} episode steps differ, e.g. {bad[:5]}"
-            print(json.dumps({"check": "ok", "episode_steps_compared": len(x)}), flush=True)
+            x = recs["reserve"]
+            assert len(x) == total_steps, len(x)
+            if "swap" in recs:
+                y = recs["swap"]
+                assert x.keys() == y.keys(), (len(x), len(y))
+                bad = [k for k in x if not torch.equal(x[k], y[k])]
+                assert not bad, f"{len(bad)} episode steps differ, e.g. {bad[:5]}"
+                print(json.dumps({"check": "ok", "run": "swap", "episode_steps_compared": len(x)}), flush=True)
+            if "recompute" in recs:
+                y = recs["recompute"]
+                assert x.keys() == y.keys(), (len(x), len(y))
+                bad = [k for k in x if not torch.equal(x[k], y[k])]
+                print(json.dumps({"check": "counted", "run": "recompute", "episode_steps_compared": len(x), "episode_steps_differing": len(bad),
+                                  "episodes_differing": len({e for e, _ in bad})}), flush=True)
 
 
 if __name__ == "__main__":

@@ -116,6 +116,7 @@ EXPORTS = [
     "vima_action_scale", "vima_action_postprocess", "vima_latent_attention", "vima_object_stats", "vima_crop_resize", "vima_head_select", "vima_gato_positions", "vima_pack_weight_f8", "vima_split_f8",
     "vima_slot_step_begin", "vima_slot_kv_append", "vima_slot_step_end", "vima_slot_kv_scatter", "vima_slot_admit_prefix",
     "vima_slot_kv_append_paged", "vima_slot_kv_scatter_paged", "vima_kv_copy_blocks", "vima_kv_pack_blocks",
+    "vima_slot_assemble_history", "vima_slot_admit_history",
     "vima_head_sample", "vima_sizeof_head_sample_desc",
 ]
 
@@ -401,6 +402,36 @@ class Context:
                                                  c_void_p(slot_mask.data_ptr()), c_void_p(len_.data_ptr()), c_void_p(n_valid.data_ptr()),
                                                  c_void_p(has_action.data_ptr()), c_void_p(active.data_ptr()), c_void_p(self._s())),
                  "slot_admit_prefix")
+
+    def slot_assemble_history(self, obs, obs_mask_u8, action, steps, P, tokens, mask, pos):
+        """obs fp32 (T, n, Q, E), obs_mask uint8 (T, n, Q) | None (every obs token valid), action fp32 (T, n, E), steps int32 [n]
+        (device) -> rows [P, L) of tokens (L, n, E) and columns [P, L) of mask uint8 / pos int64 [n, L], each episode's own history
+        (columns [0, P) of mask are read for the position base)."""
+        T, n, Q, E = obs.shape
+        L = tokens.shape[0]
+        assert steps.dtype == torch.int32 and steps.numel() == n and action.shape == (T, n, E) and tokens.shape == (L, n, E)
+        assert mask.shape == (n, L) and pos.shape == (n, L) and all(t.is_contiguous() for t in (obs, action, tokens, mask, pos, steps))
+        assert obs_mask_u8 is None or (obs_mask_u8.shape == (T, n, Q) and obs_mask_u8.is_contiguous())
+        if L == P or n == 0:  # no history column to write
+            return
+        self._ck(self.lib.vima_slot_assemble_history(self.h, c_void_p(_ptr(obs) if T else None), c_void_p(_ptr(obs_mask_u8) if T else None),
+                                                     c_void_p(_ptr(action) if T else None), c_void_p(steps.data_ptr()), int(T), int(n), int(Q),
+                                                     int(E), int(P), int(L), c_void_p(tokens.data_ptr()), c_void_p(mask.data_ptr()),
+                                                     c_void_p(pos.data_ptr()), c_void_p(self._s())), "slot_assemble_history")
+
+    def slot_admit_history(self, slots, steps, Q, P, mask, action, Lmax, slot_mask, *, len_, n_valid, has_action, active, action_token):
+        """slots / steps int32 [n] (device), mask uint8 [n, L] (assembled), action fp32 (T, n, E) -> the admitted slots' mask rows of
+        slot_mask [S, Lmax], their state (len, n_valid, has_action, active) and fed-back action rows of action_token [S, E]."""
+        n, L = mask.shape
+        T, E = action.shape[0], action.shape[2]
+        S = slot_mask.shape[0]
+        assert slots.dtype == torch.int32 and steps.dtype == torch.int32 and slots.numel() == n and steps.numel() == n
+        assert mask.is_contiguous() and action.is_contiguous() and action.shape[1] == n and action_token.shape == (S, E)
+        self._ck(self.lib.vima_slot_admit_history(self.h, c_void_p(slots.data_ptr()), c_void_p(steps.data_ptr()), int(n), int(S), int(T), int(Q),
+                                                  int(P), int(L), c_void_p(_ptr(mask) if L else None), c_void_p(_ptr(action) if T else None),
+                                                  int(E), int(Lmax), c_void_p(slot_mask.data_ptr()), c_void_p(len_.data_ptr()),
+                                                  c_void_p(n_valid.data_ptr()), c_void_p(has_action.data_ptr()), c_void_p(active.data_ptr()),
+                                                  c_void_p(action_token.data_ptr()), c_void_p(self._s())), "slot_admit_history")
 
     def kv_copy_blocks(self, bufs, row_bytes, src_row0, dst_row0, block_rows, buf_rows):
         """Block i of block_rows rows at row src_row0[i] -> row dst_row0[i] in every buffer whose base address bufs (int64 [n_buf],

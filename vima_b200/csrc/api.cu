@@ -578,6 +578,34 @@ int vima_slot_admit_prefix(vima_ctx* c, const int32_t* slots, int n, const uint8
            "slot_admit_prefix");
 }
 
+int vima_slot_assemble_history(vima_ctx* c, const float* obs, const uint8_t* obs_mask, const float* action, const int32_t* steps, int T, int n,
+                               int Q, int E, int P, int L, float* tokens, uint8_t* mask, int64_t* pos, void* stream) {
+  CHECK_CTX(c);
+  if (!steps || !tokens || !mask || !pos || (T > 0 && (!obs || !action)))
+    return fail(c, VIMA_E_INVALID, "slot_assemble_history: null pointer");
+  auto al = [](const void* q) { return ((uintptr_t)q & 15) == 0; };
+  if (T < 0 || n < 0 || Q < 1 || E < 4 || (E & 3) || P < 0 || L < P || !al(obs) || !al(action) || !al(tokens))
+    return fail(c, VIMA_E_INVALID, "slot_assemble_history: T >= 0, n >= 0, Q >= 1, E a positive multiple of 4, 0 <= P <= L, 16-byte aligned "
+                                   "obs / action / tokens");
+  LAUNCHED(c, launch_slot_assemble_history(obs, obs_mask, action, steps, T, n, Q, E, P, L, tokens, mask, (long long*)pos, (cudaStream_t)stream),
+           "slot_assemble_history");
+}
+
+int vima_slot_admit_history(vima_ctx* c, const int32_t* slots, const int32_t* steps, int n, int S, int T, int Q, int P, int L,
+                            const uint8_t* mask, const float* action, int E, int Lmax, uint8_t* slot_mask, int32_t* len, int32_t* n_valid,
+                            int32_t* has_action, int32_t* active, float* action_token, void* stream) {
+  CHECK_CTX(c);
+  if (!slots || !steps || (L > 0 && !mask) || (T > 0 && !action) || !slot_mask || !len || !n_valid || !has_action || !active || !action_token)
+    return fail(c, VIMA_E_INVALID, "slot_admit_history: null pointer");
+  auto al = [](const void* q) { return ((uintptr_t)q & 15) == 0; };
+  if (n < 0 || S < 1 || T < 0 || Q < 1 || P < 0 || L < P || L > Lmax || E < 4 || (E & 3) || !al(action) || !al(action_token))
+    return fail(c, VIMA_E_INVALID, "slot_admit_history: n >= 0, S >= 1, T >= 0, Q >= 1, 0 <= P <= L <= Lmax, E a positive multiple of 4, "
+                                   "16-byte aligned action / action_token");
+  LAUNCHED(c, launch_slot_admit_history(slots, steps, n, S, T, Q, P, L, mask, action, E, Lmax, slot_mask, len, n_valid, has_action, active,
+                                        action_token, (cudaStream_t)stream),
+           "slot_admit_history");
+}
+
 int vima_kv_copy_blocks(vima_ctx* c, void* const* bufs, int n_buf, int64_t row_bytes, const int64_t* src_row0, const int64_t* dst_row0,
                         int n_blocks, int block_rows, int64_t buf_rows, void* stream) {
   CHECK_CTX(c);

@@ -206,6 +206,13 @@ cudaError_t launch_slot_kv_scatter(const unsigned short* qkv_hi, const unsigned 
                                    int pool_pages, cudaStream_t s);
 cudaError_t launch_slot_admit_prefix(const int* slots, int n, const unsigned char* prompt_mask, int Lp, int Lmax, unsigned char* slot_mask,
                                      int* len, int* n_valid, int* has_action, int* active, cudaStream_t s);
+// Resumed slot episodes: tokens (L, n, E) rows [P, L), mask / pos [n, L] columns [P, L) of each episode's recorded history
+// (steps int32 [n] on the device; obs_mask null = every obs token valid), and the admitted slots' mask rows and state.
+cudaError_t launch_slot_assemble_history(const float* obs, const unsigned char* obs_mask, const float* action, const int* steps, int T, int n,
+                                         int Q, int E, int P, int L, float* tokens, unsigned char* mask, long long* pos, cudaStream_t s);
+cudaError_t launch_slot_admit_history(const int* slots, const int* steps, int n, int S, int T, int Q, int P, int L, const unsigned char* mask,
+                                      const float* action, int E, int Lmax, unsigned char* slot_mask, int* len, int* n_valid, int* has_action,
+                                      int* active, float* action_token, cudaStream_t s);
 // Block i of rows [src_row0[i], +block_rows) -> [dst_row0[i], +block_rows) in each of the n_buf buffers bufs[] (device array),
 // rows of row_bytes (a multiple of 16); blocks with a start outside [0, buf_rows - block_rows] are skipped.
 cudaError_t launch_kv_copy_blocks(void* const* bufs, int n_buf, long long row_bytes, const long long* src_row0, const long long* dst_row0,

@@ -196,6 +196,121 @@ cudaError_t launch_slot_admit_prefix(const int* slots, int n, const unsigned cha
   return cudaGetLastError();
 }
 
+// Admission from a recorded history (slot episodes resumed mid-way).  Episode j has completed k = steps[j] environment steps (clamped
+// to [0, T]); its history columns are forward's [o_0 (Q), a_0, o_1, ..., a_{k-2}, o_{k-1}], k(Q+1) - 1 of them (0 for k = 0),
+// placed after a prefix of P columns (decoder-only: [prompt | separator]).  Rows t >= k of obs / obs_mask / action are never read.
+__device__ __forceinline__ int slot_history_cols(const int* __restrict__ steps, int j, int T, int Q) {
+  const int k = min(max(__ldg(steps + j), 0), T);
+  return k > 0 ? k * (Q + 1) - 1 : 0;
+}
+
+// One warp per episode: mask and position ids of columns [P, L) of row j of mask / pos [n, L].  The position ids continue the
+// prefix's valid count (columns [0, P) of the same mask row, written by the caller): base + cumsum(history mask) - 1; padding
+// columns past the history get mask 0 and position id 0.
+__global__ void __launch_bounds__(32) slot_history_mask_kernel(const unsigned char* __restrict__ obs_mask, const int* __restrict__ steps, int T,
+                                                               int n, int Q, int P, int L, unsigned char* __restrict__ mask,
+                                                               long long* __restrict__ pos) {
+  const int j = blockIdx.x, lane = threadIdx.x;
+  const int hl = slot_history_cols(steps, j, T, Q);
+  unsigned char* mrow = mask + (size_t)j * L;
+  int base = 0;
+  for (int c = lane; c < P; c += 32) base += mrow[c] != 0;
+  base = __reduce_add_sync(0xffffffffu, base);
+  __syncwarp();
+  int carry = 0;
+  for (int c0 = 0; c0 < L - P; c0 += 32) {
+    const int c = c0 + lane;
+    int m = 0;
+    if (c < hl) {
+      const int t = c / (Q + 1), q = c % (Q + 1);
+      m = (q < Q && obs_mask) ? (obs_mask[((size_t)t * n + j) * Q + q] != 0) : 1;
+    }
+    int inc = m;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int y = __shfl_up_sync(0xffffffffu, inc, o);
+      if (lane >= o) inc += y;
+    }
+    if (c < L - P) {
+      mrow[P + c] = (unsigned char)m;
+      pos[(size_t)j * L + P + c] = c < hl ? (long long)(base + carry + inc - 1) : 0;
+    }
+    carry += __shfl_sync(0xffffffffu, inc, 31);
+  }
+}
+
+// Tokens (L, n, E) rows [P, L): history column c of episode j from obs (T, n, Q, E) / action (T, n, E), zero past the history.
+__global__ void slot_history_tokens_kernel(const float4* __restrict__ obs, const float4* __restrict__ act, const int* __restrict__ steps, int T,
+                                           int n, int Q, int E4, int P, int L, float4* __restrict__ tokens) {
+  const long long total = (long long)(L - P) * n * E4;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int e = (int)(i % E4);
+    const long long cj = i / E4;
+    const int j = (int)(cj % n), c = (int)(cj / n);
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (c < slot_history_cols(steps, j, T, Q)) {
+      const int t = c / (Q + 1), q = c % (Q + 1);
+      v = q < Q ? __ldg(obs + (((size_t)t * n + j) * Q + q) * E4 + e) : __ldg(act + ((size_t)t * n + j) * E4 + e);
+    }
+    tokens[((size_t)(P + c) * n + j) * E4 + e] = v;
+  }
+}
+
+cudaError_t launch_slot_assemble_history(const float* obs, const unsigned char* obs_mask, const float* action, const int* steps, int T, int n,
+                                         int Q, int E, int P, int L, float* tokens, unsigned char* mask, long long* pos, cudaStream_t s) {
+  if (n == 0 || L == P) return cudaSuccess;
+  slot_history_mask_kernel<<<n, 32, 0, s>>>(obs_mask, steps, T, n, Q, P, L, mask, pos);
+  const long long total = (long long)(L - P) * n * (E / 4);
+  const int blocks = (int)min((total + 255) / 256, (long long)132 * 16);
+  slot_history_tokens_kernel<<<blocks, 256, 0, s>>>(reinterpret_cast<const float4*>(obs), reinterpret_cast<const float4*>(action), steps, T, n,
+                                                    Q, E / 4, P, L, reinterpret_cast<float4*>(tokens));
+  return cudaGetLastError();
+}
+
+// One block per episode j, slot b = slots[j] (skipped outside [0, S), or when its P + history columns exceed L): mask row b of
+// slot_mask [S, Lmax] <- columns [0, len) of mask row j, 0 past them; len = P + history columns, n_valid = valid columns of
+// [0, len), has_action = (k > 0), active = 1, and for k > 0 the fed-back action row action_token[b] <- action[k-1, j].
+__global__ void __launch_bounds__(256) slot_admit_history_kernel(const int* __restrict__ slots, const int* __restrict__ steps, int S, int T,
+                                                                 int n, int Q, int P, int L, const unsigned char* __restrict__ mask,
+                                                                 const float4* __restrict__ action, int E4, int Lmax,
+                                                                 unsigned char* __restrict__ slot_mask, int* __restrict__ len,
+                                                                 int* __restrict__ n_valid, int* __restrict__ has_action,
+                                                                 int* __restrict__ active, float4* __restrict__ action_token) {
+  __shared__ int warp_cnt[8];
+  const int j = blockIdx.x, b = __ldg(slots + j);
+  const int k = min(max(__ldg(steps + j), 0), T);
+  const int ln = P + slot_history_cols(steps, j, T, Q);
+  if (b < 0 || b >= S || ln > L) return;
+  int cnt = 0;
+  for (int c = threadIdx.x; c < Lmax; c += blockDim.x) {
+    const unsigned char m = c < ln ? (mask[(size_t)j * L + c] != 0) : 0;
+    slot_mask[(size_t)b * Lmax + c] = m;
+    cnt += m;
+  }
+  if (k > 0)
+    for (int e = threadIdx.x; e < E4; e += blockDim.x) action_token[(size_t)b * E4 + e] = __ldg(action + ((size_t)(k - 1) * n + j) * E4 + e);
+  cnt = __reduce_add_sync(0xffffffffu, cnt);
+  if ((threadIdx.x & 31) == 0) warp_cnt[threadIdx.x >> 5] = cnt;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int total = 0;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) total += warp_cnt[w];
+    len[b] = ln;
+    n_valid[b] = total;
+    has_action[b] = k > 0;
+    active[b] = 1;
+  }
+}
+
+cudaError_t launch_slot_admit_history(const int* slots, const int* steps, int n, int S, int T, int Q, int P, int L, const unsigned char* mask,
+                                      const float* action, int E, int Lmax, unsigned char* slot_mask, int* len, int* n_valid, int* has_action,
+                                      int* active, float* action_token, cudaStream_t s) {
+  if (n == 0) return cudaSuccess;
+  slot_admit_history_kernel<<<n, 256, 0, s>>>(slots, steps, S, T, n, Q, P, L, mask, reinterpret_cast<const float4*>(action), E / 4, Lmax,
+                                              slot_mask, len, n_valid, has_action, active, reinterpret_cast<float4*>(action_token));
+  return cudaGetLastError();
+}
+
 // Block copies between rows of the same buffers (copy on write of shared K/V pages, a fork's prompt K/V rows).  Grid (row chunk,
 // block, buffer): block i of buffer z, rows [src_row0[i], +block_rows) -> rows [dst_row0[i], +block_rows), 16 bytes per thread and
 // trip.  The block's rows are contiguous (pitch = row_bytes), so each block is one flat copy.  A block with either start outside

@@ -380,15 +380,16 @@ class SlotDecodeCache:
                 raise ValueError(f"admitting {len(slots)} prompts of {prompt_cols} tokens needs {need} prompt pages, {have} are free: "
                                  "release slots or open the cache with a larger prompt_pool_tokens")
 
-    def free_slots(self, slots: list, prefix_cols: int = 0, prompt_cols: int = 0) -> None:
-        """Return the pages of `slots` (released or re-admitted), history and prompt, and give each `prefix_cols` columns of new
-        history pages and `prompt_cols` columns of new prompt pages (checked by check_prefix), the rows of the last prompt page past
-        `prompt_cols` zeroed.  Asynchronous, no host synchronisation."""
+    def free_slots(self, slots: list, prefix_cols=0, prompt_cols: int = 0) -> None:
+        """Return the pages of `slots` (released or re-admitted), history and prompt, and give each `prefix_cols` columns (an int, or
+        one per slot) of new history pages and `prompt_cols` columns of new prompt pages (checked by check_prefix or
+        check_admit_history), the rows of the last prompt page past `prompt_cols` zeroed.  Asynchronous, no host synchronisation."""
+        cols = prefix_cols if isinstance(prefix_cols, list) else [prefix_cols] * len(slots)
         upd = []
         for b in slots:
             upd += self.pages.release(b)
-        for b in slots:
-            upd += self.pages.reserve(b, prefix_cols)
+        for b, c in zip(slots, cols):
+            upd += self.pages.reserve(b, c)
         self._push_pages(upd)
         if self.Lp_cap:
             upd = []
@@ -453,6 +454,37 @@ class SlotDecodeCache:
             t.index_copy_(0, di, t.index_select(0, si))
         for a, b in zip(src, dst):
             self.len_host[b], self.has_action_host[b], self.active_host[b] = self.len_host[a], self.has_action_host[a], True
+
+    # ---- resumed episodes: a slot admitted mid-way from its recorded history (DESIGN.md 7 (f)1)
+    def check_admit_history(self, slots: list, lens: list, prompt_cols: int = 0) -> None:
+        """Everything on the cache's side that can refuse admitting slots[j] at lens[j] cache columns (prefix and history) with
+        (cross-attention policies) a prompt of `prompt_cols` tokens, before any state is touched: a length past Lmax, and pools that
+        cannot cover ceil(lens[j]/64) history pages each and ceil(prompt_cols/64) prompt pages each, counting the pages the
+        destinations give back (a page still shared with a slot outside `slots` is not given back)."""
+        over = [(b, c) for b, c in zip(slots, lens) if not 0 <= c <= self.Lmax]
+        if over:
+            raise ValueError(f"admit_history: (slot, history columns) {over} do not fit max_tokens={self.Lmax}")
+        need = sum(self.pages.pages_for(c) for c in lens)
+        have = self.kv_pages_free + self.pages.freed_by(slots)
+        if need > have:
+            raise ValueError(f"admit_history: {len(slots)} histories of {list(lens)} columns need {need} K/V pages, {have} are free: "
+                             "release or swap out slots, or open the cache with a larger kv_pool_tokens")
+        if self.Lp_cap:
+            need = len(slots) * self.prompt_pages.pages_for(prompt_cols)
+            have = self.prompt_pages_free + self.prompt_pages.freed_by(slots)
+            if need > have:
+                raise ValueError(f"admit_history: {len(slots)} prompts of {prompt_cols} tokens need {need} prompt pages, {have} are free: "
+                                 "release or swap out slots, or open the cache with a larger prompt_pool_tokens")
+
+    def reserve_history(self, slots: list, lens: list, has_action: list, prompt_cols: int = 0) -> None:
+        """The page-taking step of a history admission (after check_admit_history, so it cannot fail): the destinations let go of
+        their pages (a live episode is replaced; a page a fork still holds stays with it), slots[j] takes ceil(lens[j]/64) private
+        history pages and ceil(prompt_cols/64) prompt pages, the table rows are pushed, and the host mirrors become len = lens[j],
+        has_action[j], active.  The device rows and state are written by the prefill that follows.  Asynchronous, no host
+        synchronisation."""
+        self.free_slots(slots, list(lens), prompt_cols)
+        for b, c, a in zip(slots, lens, has_action):
+            self.len_host[b], self.has_action_host[b], self.active_host[b] = int(c), bool(a), True
 
     # ---- swapped episodes: a slot's episode to pinned host memory and back (DESIGN.md 7 (f)1)
     def swap_key(self) -> tuple:
@@ -948,17 +980,67 @@ class XAttnGPT(nn.Module):
         cache.free_slots(slots, prompt_cols=Lp)
         idx = cache.device_ints(slots)
         sl = idx.to(torch.int32)
-        for W, khi, klo in zip(self._packed(ctx, p), cache.prompt_kv_hi, cache.prompt_kv_lo):
-            kv = eng.gemm(ctx, kv16, W["wkv"], p, want16=True)[1]
-            ctx.slot_kv_scatter_paged(kv.hi, kv.lo, kv.ld, 0, 2 * E, n, Lp, sl, khi, klo, 2 * E, cache.prompt_page_table,
-                                      cache.prompt_pages.n_pages)
-        cache.prompt_mask.index_fill_(0, idx, 0)
-        cache.prompt_mask[idx, :Lp] = prompt_mask_u8
-        cache.prompt_len.index_fill_(0, idx, Lp)
+        for i, W in enumerate(self._packed(ctx, p)):
+            self._scatter_prompt_kv(ctx, cache, sl, eng.gemm(ctx, kv16, W["wkv"], p, want16=True)[1], i, n, Lp, E)
+        self._set_prompt_rows(cache, idx, prompt_mask_u8, Lp)
         for t, v in ((cache.len, 0), (cache.n_valid, 0), (cache.has_action, 0), (cache.active, 1)):
             t.index_fill_(0, idx, v)
         for b in slots:
             cache.len_host[b], cache.has_action_host[b], cache.active_host[b] = 0, False, True
+
+    @staticmethod
+    def _scatter_prompt_kv(ctx, cache: SlotDecodeCache, sl: torch.Tensor, kv: "eng.Opnd", layer: int, n: int, Lp: int, E: int) -> None:
+        """Layer `layer`'s projected prompt keys/values kv [n*Lp, 2E] -> the prompt pages of slots sl (int32 [n], device)."""
+        ctx.slot_kv_scatter_paged(kv.hi, kv.lo, kv.ld, 0, 2 * E, n, Lp, sl, cache.prompt_kv_hi[layer], cache.prompt_kv_lo[layer], 2 * E,
+                                  cache.prompt_page_table, cache.prompt_pages.n_pages)
+
+    @staticmethod
+    def _set_prompt_rows(cache: SlotDecodeCache, idx: torch.Tensor, prompt_mask_u8: torch.Tensor, Lp: int) -> None:
+        """Prompt mask rows (padded to Lp_cap with masked columns) and prompt length of the admitted slots idx (int64, device)."""
+        cache.prompt_mask.index_fill_(0, idx, 0)
+        cache.prompt_mask[idx, :Lp] = prompt_mask_u8
+        cache.prompt_len.index_fill_(0, idx, Lp)
+
+    @torch.no_grad()
+    def prefill_history(self, cache: SlotDecodeCache, slots: list, tokens: torch.Tensor, mask_u8: torch.Tensor, position_ids: torch.Tensor,
+                        prompt_tokens: torch.Tensor, prompt_mask_u8: torch.Tensor, prompt_position_ids: torch.Tensor, steps: torch.Tensor,
+                        actions: torch.Tensor, Q: int) -> None:
+        """Slot episodes admitted mid-way (after cache.reserve_history gave slots[j] its pages): tokens (L,n,E) hold each episode's
+        recorded history as vima_slot_assemble_history lays it out (mask / position ids (n,L), padding columns masked), prompt_tokens
+        (Lp,n,E) / prompt mask / position ids (n,Lp) its prompt.  One pass of forward's arithmetic over the n*L rows: each layer's
+        key_value GEMM of the prompts feeds the cross-attention and is scattered into the slots' prompt pages (as admit_prompts does),
+        and each causal block's keys / values go to the slots' history pages (run_block kv_scatter; columns past a slot's pages land
+        on the zero page and are skipped).  Then vima_slot_admit_history writes the mask rows, state and fed-back actions (steps int32
+        [n] on the device, actions (T,n,E)).  With L = 0 (no history) only the prompt is projected, as admit_prompts does.  The caller
+        has validated everything; no host synchronisation."""
+        L, n, E = tokens.shape
+        Lp = prompt_tokens.shape[0]
+        ctx = eng.ctx_for(prompt_tokens)
+        p = eng.prec()
+        dev = prompt_tokens.device
+        self._pos_guard.poll()
+        err = self._pos_guard.device_flag(dev)  # a bad position id is reported by the next step
+        kv16 = self._prompt_operand(ctx, p, prompt_tokens.float(), prompt_position_ids, False, n, Lp, E, err)
+        idx = cache.device_ints(slots)
+        sl = idx.to(torch.int32)
+
+        def prompt_kv(i, W):
+            kv = eng.gemm(ctx, kv16, W["wkv"], p, want16=True)[1]
+            self._scatter_prompt_kv(ctx, cache, sl, kv, i, n, Lp, E)
+            return kv.hi, kv.lo, kv.ld, {}
+
+        if L == 0:
+            for i, W in enumerate(self._packed(ctx, p)):
+                prompt_kv(i, W)
+        else:
+            x32 = torch.empty((n * L, E), dtype=torch.float32, device=dev)
+            ctx.add_pos_embed(tokens, tokens.stride(1), tokens.stride(0), position_ids, self.positions_embed.weight.detach(), n, L, E,
+                              out_f32=x32, err_flag=err)
+            self._layers(ctx, p, x32, B=n, L=L, E=E, Lp=Lp, omask=mask_u8, pmask=prompt_mask_u8, prompt_kv=prompt_kv,
+                         kv_scatter=(sl, cache))
+        self._set_prompt_rows(cache, idx, prompt_mask_u8, Lp)
+        ctx.slot_admit_history(sl, steps, Q, 0, mask_u8, actions, cache.Lmax, cache.mask, len_=cache.len, n_valid=cache.n_valid,
+                               has_action=cache.has_action, active=cache.active, action_token=cache.action_token)
 
     # ---------------------------------------------------------------------------------------------
     def forward(
@@ -1031,21 +1113,38 @@ class XAttnGPT(nn.Module):
             self._input_checked = True
 
         layers = self._packed(ctx, p)
+        if cache is not None and need_prompt:
+            cache.prompt_kv = [eng.gemm(ctx, kv16, W["wkv"], p, want16=True)[1] for W in layers]
+
+        def prompt_kv(i, W):
+            if slots:  # each slot's prompt through its page table, prompt_len[b] keys
+                return cache.prompt_kv_hi[i], cache.prompt_kv_lo[i], 2 * E, dict(kv_pages=cache.prompt_page_table,
+                                                                                 kv_pool_pages=cache.prompt_pages.n_pages, kv_len=cache.prompt_len)
+            kvp16 = cache.prompt_kv[i] if cache is not None else eng.gemm(ctx, kv16, W["wkv"], p, want16=True)[1]
+            return kvp16.hi, kvp16.lo, kvp16.ld, {}
+
+        x32 = self._layers(ctx, p, x32, B=B, L=L, E=E, Lp=Lp, omask=omask, pmask=pmask, prompt_kv=prompt_kv, cache=cache)
+        if cache is not None and not slots:
+            cache.L += L
+        out = x32.view(B, L, E)
+        return out if batch_first else out.transpose(0, 1)
+
+    def _layers(self, ctx, p, x32, *, B, L, E, Lp, omask, pmask, prompt_kv, cache=None, kv_scatter=None) -> torch.Tensor:
+        """The decoder stack over the residual stream x32 [B*L, E] (tokens + position embeddings) -> the last block's output [B*L, E]:
+        per layer cross-attention to the prompt keys/values prompt_kv(layer, packed weights) -> (hi, lo, ld, paged attention
+        arguments) under the key mask pmask, then the causal block (run_block with `cache` / `kv_scatter`)."""
+        M, H, Hx = B * L, self.n_head, self.xattn_n_head
+        d_x = E // Hx
+        dev = x32.device
+        layers = self._packed(ctx, p)
         lnw = lambda ln: (ln.weight.detach(), ln.bias.detach())
         # first layer's query LayerNorm; later ones are chained onto the previous block's LN2
         w, b = lnw(self.xattns[0].layernorm)
         _, _, qin16 = eng.norm(ctx, x32, p, rows=M, cols=E, w=w, b=b, eps=self.xattns[0].layernorm.eps, want16=True, out_f8=True)
-        if cache is not None and need_prompt:
-            cache.prompt_kv = [eng.gemm(ctx, kv16, W["wkv"], p, want16=True)[1] for W in layers]
         for i, (blk, xa, W) in enumerate(zip(self.h, self.xattns, layers)):
             # ---------------- XAttention ----------------
             _, q16 = eng.gemm(ctx, qin16, W["wq"], p, want16=True)
-            if slots:  # each slot's prompt through its page table, prompt_len[b] keys
-                khi, klo, kld = cache.prompt_kv_hi[i], cache.prompt_kv_lo[i], 2 * E
-                paged = dict(kv_pages=cache.prompt_page_table, kv_pool_pages=cache.prompt_pages.n_pages, kv_len=cache.prompt_len)
-            else:
-                kvp16 = cache.prompt_kv[i] if cache is not None else eng.gemm(ctx, kv16, W["wkv"], p, want16=True)[1]
-                khi, klo, kld, paged = kvp16.hi, kvp16.lo, kvp16.ld, {}
+            khi, klo, kld, paged = prompt_kv(i, W)
             c16 = eng.Opnd(M, E, dev, p.split, f8=p.f8)
             ctx.attention(q=(q16.hi, q16.lo, q16.ld, 0), k=(khi, klo, kld, 0), v=(khi, klo, kld, E), o=(c16.hi, c16.lo, c16.ld, 0), B=B,
                           H=Hx, Lq=L, Lk=Lp, D=d_x, scale=1.0 / math.sqrt(d_x), causal=False, key_mask=pmask, dtype=p.dtype,
@@ -1059,11 +1158,8 @@ class XAttnGPT(nn.Module):
             # ---------------- causal Block ----------------
             nxt = self.xattns[i + 1].layernorm if i + 1 < self.n_layer else None
             x32, qin16 = run_block(ctx, p, W, blk, xb32, xb16, c16, B=B, L=L, E=E, H=H, omask=omask, chain_ln=nxt, out_f32=x32, cache=cache,
-                                   layer=i)
-        if cache is not None and not slots:
-            cache.L += L
-        out = x32.view(B, L, E)
-        return out if batch_first else out.transpose(0, 1)
+                                   layer=i, kv_scatter=kv_scatter)
+        return x32
 
 
 class _OpenAIGPTModel(nn.Module):
@@ -1135,25 +1231,35 @@ class HFGPT(nn.Module):
         return out
 
     @torch.no_grad()
-    def prefill(self, cache, slots: list, x: torch.Tensor, custom_mask_u8: torch.Tensor, position_ids: torch.Tensor) -> None:
+    def prefill(self, cache, slots: list, x: torch.Tensor, custom_mask_u8: torch.Tensor, position_ids: torch.Tensor, history=None) -> None:
         """Decoder-only prompt prefill.  x (L,n,E) holds n new sequences [prompt | separator] (custom_mask_u8 / position_ids (n,L);
         the separator, last, is valid).  They run through every block with local causal attention -- the arithmetic of `forward` --
         and after each layer's c_attn GEMM their keys / values go to cache columns [0, L) of slots[j] (vima_slot_kv_scatter; into the
         pages the slots take first for a SlotDecodeCache, whose earlier pages go back to the pool).  Then the mask columns [0, L)
         and the state are set: a SlotDecodeCache's by vima_slot_admit_prefix (len = L, n_valid = valid tokens, no action, active), a
         DecodeCache's (slots = all its rows, in order) by copying the mask and setting L and n_valid.  The caller has validated
-        shapes, slots, capacity (for a SlotDecodeCache also check_prefix) and the precision mode."""
+        shapes, slots, capacity (for a SlotDecodeCache also check_prefix) and the precision mode.
+
+        With `history` = (steps int32 [n] on the device, actions (T,n,E), Q, P) the n sequences are [prompt | separator | recorded
+        history] of slot episodes admitted mid-way, padded to the longest (vima_slot_assemble_history; P = Lp+1 prefix columns, padding
+        columns masked): the caller has taken their pages (SlotDecodeCache.reserve_history; padding columns past a slot's pages land
+        on the zero page and are skipped), and vima_slot_admit_history sets the mask rows, state and fed-back actions."""
         eng.uses(self)  # fp32 parameters read by the kernels directly
         ctx = eng.ctx_for(x)
         p = eng.prec()
         L, n, E = x.shape
         if isinstance(cache, SlotDecodeCache):
-            cache.free_slots(slots, L)
+            if history is None:
+                cache.free_slots(slots, L)
             sl = cache.device_ints(slots).to(torch.int32)
         else:
             sl = torch.tensor(slots, dtype=torch.int32, device=x.device)
         self._stack(ctx, p, x, custom_mask_u8, position_ids, False, kv_scatter=(sl, cache))
-        if isinstance(cache, SlotDecodeCache):
+        if history is not None:
+            steps, actions, Q, P = history
+            ctx.slot_admit_history(sl, steps, Q, P, custom_mask_u8, actions, cache.Lmax, cache.mask, len_=cache.len, n_valid=cache.n_valid,
+                                   has_action=cache.has_action, active=cache.active, action_token=cache.action_token)
+        elif isinstance(cache, SlotDecodeCache):
             ctx.slot_admit_prefix(sl, custom_mask_u8[:, :L - 1].contiguous(), cache.Lmax, cache.mask, len_=cache.len, n_valid=cache.n_valid,
                                   has_action=cache.has_action, active=cache.active)
             for b in slots:

@@ -110,6 +110,14 @@ class VIMAFlamingoPolicy(VIMAGatoPolicy):
         eng.ctx_for(prompt_token)
         return VIMAPolicy.admit(self, cache, slots, prompt_token, prompt_token_mask)
 
+    def admit_history(self, cache, slots, prompt_token: torch.Tensor, prompt_token_mask: torch.Tensor, obs_token: torch.Tensor,
+                      action_token: torch.Tensor, steps) -> None:
+        """VIMAPolicy.admit_history with every obs token valid: obs_token (T,n,Q,E), action_token (T,n,E), steps n host ints."""
+        eng.ctx_for(prompt_token)
+        if obs_token.dim() == 4:
+            self._check_obs(obs_token.shape[2])
+        return VIMAPolicy._admit_history(self, cache, slots, prompt_token, prompt_token_mask, obs_token, None, action_token, steps)
+
     release = VIMAPolicy.release
     fork_slots = VIMAPolicy.fork_slots
     swap_out = VIMAPolicy.swap_out

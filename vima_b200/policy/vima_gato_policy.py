@@ -15,7 +15,7 @@ import torch.nn as nn
 from .. import engine as eng
 from .. import nn as vnn
 from ..utils import *  # noqa: F401,F403
-from .vima_policy import VIMAPolicy
+from .vima_policy import VIMAPolicy, history_cols, history_steps
 
 
 class VIMAGatoPolicy(nn.Module):
@@ -195,6 +195,38 @@ class VIMAGatoPolicy(nn.Module):
         if not s:
             return
         self.transformer.prefill(cache, s, *self._prompt_prefix(ctx, prompt_token, prompt_token_mask))
+
+    def admit_history(self, cache, slots, prompt_token: torch.Tensor, prompt_token_mask: torch.Tensor, obs_token: torch.Tensor,
+                      action_token: torch.Tensor, steps) -> None:
+        """VIMAPolicy.admit_history with every obs token valid: obs_token (T,n,Q,E), action_token (T,n,E), steps n host ints in
+        [0, T].  Slot slots[j]'s columns become [prompt | separator | o_0, a_0, ..., o_{k-1}] (k = steps[j]), the first
+        Lp + 1 + k(Q+1) - 1 tokens of `forward`, prefilled in one batched pass over the decoder."""
+        s = cache.slot_index(slots)
+        if cache.Lp_cap:
+            raise ValueError("admit_history: this SlotDecodeCache was opened for a cross-attention decoder")
+        self._check_prompt(prompt_token, prompt_token_mask, len(s), cache.Lmax)
+        k, T, Q = history_steps(cache, s, obs_token, None, action_token, steps)
+        self._check_obs(Q)
+        Lp, n, E = prompt_token.shape
+        lens = [Lp + 1 + history_cols(x, Q) for x in k]
+        cache.check_precision(eng.prec())
+        cache.check_admit_history(s, lens)
+        if not s:
+            return
+        ctx = eng.ctx_for(prompt_token)
+        dev = prompt_token.device
+        cache.reserve_history(s, lens, [x > 0 for x in k])
+        steps32 = cache.device_ints(k).to(torch.int32)
+        act = action_token.float().contiguous()
+        L = max(lens)
+        tokens = torch.empty((L, n, E), dtype=torch.float32, device=dev)
+        tokens[:Lp].copy_(prompt_token)
+        tokens[Lp].copy_(self.prompt_sep_token.detach().unsqueeze(0).expand(n, E))
+        mask = torch.empty((n, L), dtype=torch.uint8, device=dev)
+        pos = torch.empty((n, L), dtype=torch.int64, device=dev)
+        ctx.gato_positions(eng.as_u8(prompt_token_mask).contiguous(), L, mask, pos)  # columns [0, Lp+1); the rest is the history's
+        ctx.slot_assemble_history(obs_token.float().contiguous(), None, act, steps32, Lp + 1, tokens, mask, pos)
+        self.transformer.prefill(cache, s, tokens, mask, pos, history=(steps32, act, Q, Lp + 1))
 
     release = VIMAPolicy.release
     fork_slots = VIMAPolicy.fork_slots

@@ -71,6 +71,11 @@ class VIMAGPTPolicy(VIMAGatoPolicy):
         """obs_token (1,B,E), prev_action_token (1,B,E) (None at the first step) -> (1,B,E)."""
         return VIMAGatoPolicy.forward_step(self, cache, obs_token.unsqueeze(2), prev_action_token)
 
+    def admit_history(self, cache, slots, prompt_token: torch.Tensor, prompt_token_mask: torch.Tensor, obs_token: torch.Tensor,
+                      action_token: torch.Tensor, steps) -> None:
+        """obs_token (T,n,E), action_token (T,n,E), steps n host ints: VIMAGatoPolicy.admit_history with one token per observation."""
+        return VIMAGatoPolicy.admit_history(self, cache, slots, prompt_token, prompt_token_mask, obs_token.unsqueeze(2), action_token, steps)
+
     def step_slots(self, cache, obs_token: torch.Tensor, action_token: Optional[torch.Tensor]) -> torch.Tensor:
         """obs_token (1,S,E), action_token (1,S,E) | None -> (1,S,E)."""
         return VIMAGatoPolicy.step_slots(self, cache, obs_token.unsqueeze(2), action_token)

@@ -18,6 +18,32 @@ from .. import nn as vnn
 from ..utils import *  # noqa: F401,F403  (the reference re-exports vima.utils here)
 
 
+def history_steps(cache, s: list, obs_token: torch.Tensor, obs_mask: Optional[torch.Tensor], action_token: torch.Tensor, steps) -> tuple:
+    """admit_history's checks of a recorded history for the destination slots `s` (before any state is touched): obs_token
+    (T,n,Q,E), obs_mask (T,n,Q) or None, action_token (T,n,E), steps n host ints in [0, T] -> (steps as a list of ints, T, Q)."""
+    if isinstance(steps, torch.Tensor):
+        if steps.device.type != "cpu":
+            raise TypeError("admit_history: steps must be host ints (a device tensor would need a synchronising read)")
+        steps = steps.tolist()
+    k = [int(x) for x in steps]
+    n, E = len(s), cache.E
+    if obs_token.dim() != 4 or obs_token.shape[1] != n or obs_token.shape[3] != E or obs_token.shape[2] < 1:
+        raise ValueError(f"admit_history: {n} slots need obs_token (T, {n}, Q, {E}), got {tuple(obs_token.shape)}")
+    T, _, Q, _ = obs_token.shape
+    if obs_mask is not None and tuple(obs_mask.shape) != (T, n, Q):
+        raise ValueError(f"admit_history: obs_mask must be ({T}, {n}, {Q}), got {tuple(obs_mask.shape)}")
+    if tuple(action_token.shape) != (T, n, E):
+        raise ValueError(f"admit_history: action_token must be ({T}, {n}, {E}), got {tuple(action_token.shape)}")
+    if len(k) != n or any(not 0 <= x <= T for x in k):
+        raise ValueError(f"admit_history: steps must be {n} ints in [0, T={T}], got {k}")
+    return k, T, Q
+
+
+def history_cols(k: int, Q: int) -> int:
+    """Cache columns of k completed environment steps at obs width Q: [o_0, a_0, ..., a_{k-2}, o_{k-1}]."""
+    return k * (Q + 1) - 1 if k else 0
+
+
 class VIMAPolicy(nn.Module):
     def __init__(self, *, embed_dim: int, xf_n_layers: int, sattn_n_heads: int, xattn_n_heads: int):
         super().__init__()
@@ -234,6 +260,56 @@ class VIMAPolicy(nn.Module):
         s, eps = cache.check_swap_in(slots, episodes)
         cache.check_precision(eng.prec())
         cache.swap_in(s, eps)
+
+    def admit_history(self, cache, slots, prompt_token: torch.Tensor, prompt_token_mask: torch.Tensor, obs_token: torch.Tensor,
+                      obs_mask: torch.Tensor, action_token: torch.Tensor, steps) -> None:
+        """Start each of `slots` (replacing whatever it held) mid-way through an episode whose history was recorded: prompt_token
+        (Lp,n,E) / prompt_token_mask (n,Lp) as in `admit`, obs_token (T,n,Q,E), obs_mask (T,n,Q), action_token (T,n,E) (the embedding
+        of the action taken after each observation), steps n host ints: episode j has completed steps[j] <= T environment steps.
+        Rows t >= steps[j] are never read (they may hold anything), so episodes of different lengths share one call, padded to the
+        longest.  Afterwards slot slots[j] holds episode j as if it had been admitted and stepped steps[j] times at width Q (a history
+        stepped at other widths is re-padded to Q: padded obs tokens are masked keys that do not advance position ids); its next
+        step feeds [a_{k-1}, o_k] and act_slots feeds back action_token[steps[j] - 1, j].  One batched prefill pass over the decoder
+        (forward's arithmetic over n x the longest history), so the resumed K/V match the stepped ones within the bars of
+        forward_step, not bit for bit.  Uses: resuming preempted episodes by recomputation instead of swapping, carrying running
+        episodes across a weight update (open a new cache and admit their histories), starting from a recorded trajectory.  Refuses
+        (ValueError, nothing touched) bad or repeated slots, shapes or steps, histories past max_tokens, prompts past
+        max_prompt_tokens, pools that cannot cover the pages (counting those the destinations give back), and a cache of another
+        precision mode or of changed weights; steps on the device raise TypeError.  Queued on the current stream, no host
+        synchronisation."""
+        self._admit_history(cache, slots, prompt_token, prompt_token_mask, obs_token, obs_mask, action_token, steps)
+
+    def _admit_history(self, cache, slots, prompt_token, prompt_token_mask, obs_token, obs_mask, action_token, steps) -> None:
+        """admit_history of the cross-attention policies (obs_mask None: every obs token valid)."""
+        s = cache.slot_index(slots)
+        k, T, Q = history_steps(cache, s, obs_token, obs_mask, action_token, steps)
+        Lp, n, E = prompt_token.shape
+        if not cache.Lp_cap:
+            raise ValueError("admit_history: this SlotDecodeCache was opened for a decoder-only policy")
+        if n != len(s) or E != cache.E or tuple(prompt_token_mask.shape) != (n, Lp):
+            raise ValueError(f"admit_history: {len(s)} slots need prompt_token (Lp, {len(s)}, {cache.E}) and a ({len(s)}, Lp) mask, got "
+                             f"{tuple(prompt_token.shape)} / {tuple(prompt_token_mask.shape)}")
+        if Lp > cache.Lp_cap:
+            raise ValueError(f"admit_history: prompt of {Lp} tokens exceeds the cache's max_prompt_tokens={cache.Lp_cap}")
+        lens = [history_cols(x, Q) for x in k]
+        cache.check_precision(eng.prec())
+        cache.check_admit_history(s, lens, Lp)
+        if not s:
+            return
+        ctx = eng.ctx_for(prompt_token)
+        dev = prompt_token.device
+        cache.reserve_history(s, lens, [x > 0 for x in k], Lp)
+        steps32 = cache.device_ints(k).to(torch.int32)
+        obs = obs_token.float().contiguous()
+        act = action_token.float().contiguous()
+        L = max(lens)
+        tokens = torch.empty((L, n, E), dtype=torch.float32, device=dev)
+        mask = torch.empty((n, L), dtype=torch.uint8, device=dev)
+        pos = torch.empty((n, L), dtype=torch.int64, device=dev)
+        ctx.slot_assemble_history(obs, None if obs_mask is None else eng.as_u8(obs_mask), act, steps32, 0, tokens, mask, pos)
+        pmask_u8 = eng.as_u8(prompt_token_mask)
+        self.xattn_gpt.prefill_history(cache, s, tokens, mask, pos, prompt_token, pmask_u8, self._prompt_positions(ctx, pmask_u8), steps32,
+                                       act, Q)
 
     def step_slots(self, cache, obs_token: torch.Tensor, obs_mask: torch.Tensor, action_token: Optional[torch.Tensor]) -> torch.Tensor:
         """One environment step of every slot: obs_token (1,S,Q,E), obs_mask (1,S,Q), action_token (1,S,E) (the previous action of
