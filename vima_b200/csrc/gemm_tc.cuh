@@ -28,7 +28,7 @@ constexpr int GEMM_PRODUCER_REGS = 40;              // setmaxnreg split of the 6
 constexpr int GEMM_CONSUMER_REGS = 232;
 constexpr int GEMM_MAX_BN = 128;                    // 64 fp32 accumulator registers per thread and accumulator
 constexpr int GEMM_MAX_STAGES = 8;
-constexpr int GEMM_STAGING_BYTES = 8 * 16 * 16 * 4;  // per-consumer-warp 16x16 fp32 transpose buffers (XOR-swizzled)
+constexpr int GEMM_STAGING_BYTES = 8 * 16 * 32 * 4;  // per-consumer-warp 16x32 fp32 transpose buffers (XOR-swizzled)
 
 struct alignas(64) GemmParams {
   CUtensorMap tm_a_hi, tm_a_lo, tm_b_hi, tm_b_lo;  // in mode 2: tm_a_lo = A_lo8, tm_b_lo = B_lo8
@@ -108,14 +108,22 @@ __device__ __forceinline__ void acc_group16(const float (&acc)[BN / 2], int s, f
     }
 }
 
-// One accumulator tile, this warp's share: rows [row_base, +16) x every column.  Per 16-column sub-chunk: fragment registers
-// -> bias/act/GLU -> smem transpose (16x16 floats, 16-byte chunks XOR-swizzled by (row>>1)&3) -> [8 rows x 4 lanes x float4]
-// -> mul / residual / stores (128-bit fp32, 64-bit 16-bit pairs), issued after the sub-chunk's global loads are already in flight.
-// Row statistics keep the two column halves of the original layout: part 2*tn + ((column / 32) & 1).
+// One accumulator tile, this warp's share: rows [row_base, +16) x every column, in 32-column chunks.  Per chunk: fragment registers
+// -> bias/act/GLU -> smem transpose (16 x 32 floats, 16-byte chunks XOR-swizzled by 2 * (row & 3)) -> [4 rows x 8 lanes x float4]
+// -> mul / residual / stores.  Each store instruction covers 4 rows of whole 32-byte sectors: a 128-byte line per row of fp32,
+// 64 bytes of fp16 and 32 bytes of each e4m3 view.  The multiplier / residual rows of every chunk (NB chunks in the generic variant)
+// are requested together before the first chunk is processed, so the tile waits out one L2 round trip instead of one per chunk.
+// Row statistics keep the two column halves of the original layout: part 2*tn + ((column / 32) & 1), i.e. the chunk's parity.  The
+// even chunks run first, then the odd ones, so each half's sums are complete before the other's start.  The summation tree is that of
+// 16-column sub-chunks: per row and 4-column group kc, the sub-chunks of the half in ascending order (columns 4kc.. of a chunk are
+// lane c8 = kc, columns 16 + 4kc.. lane kc + 4), then the xor-1 / xor-2 fold over kc.
 // acc is the m64nNk16 fragment: element 4*g + e holds column 8*g + 2*(lane % 4) + (e & 1), row 8*(e >> 1) + lane / 4.
 template <class E, int BN>
 __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float (&acc)[BN / 2], const float* __restrict__ sb,
                                               float* __restrict__ st, int lane, int row_base, int tn, int bn_out, int n_out) {
+  constexpr int NCH = BN / 32;                                // 32-column chunks (bn_out is a multiple of 32 too)
+  constexpr int NEV = (NCH + 1) / 2;                          // even chunks: statistics half 0
+  constexpr int NB = E::GENERIC ? (NCH < 2 ? NCH : 2) : NCH;  // chunks whose mul / residual rows are in registers together
   const bool glu = E::GENERIC ? (p.glu != 0) : E::GLU;
   const bool has_mul = E::GENERIC ? (p.mul != nullptr) : E::MUL;
   const bool has_res = E::GENERIC ? (p.residual != nullptr) : E::RES;
@@ -125,8 +133,10 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float (
   const bool lnr = E::GENERIC ? (p.res_stats != nullptr) : E::LNR;
   const bool stats = E::GENERIC ? (p.stats_out != nullptr) : E::STATS;
   const float scale = p.acc_scale;
-  const int sub = lane >> 2;        // row within a group of 8 (transposed layout); also the fragment row
-  const int kc = lane & 3;          // which 4-column group of the 16-column sub-chunk; also the fragment column pair
+  const int sub = lane >> 2;        // fragment row within a group of 8
+  const int kc = lane & 3;          // fragment column pair
+  const int rq = lane >> 3;         // transposed layout: row within a group of 4 (rows 4*it + rq)
+  const int c8 = lane & 7;          // transposed layout: 4-column group of the chunk
   const float* sc1 = sb + 256;      // ln_c1 tile (accumulator-column order, like the bias tile)
   const float* sgam = sb + 512;     // res_gamma / res_beta tiles (output-column order)
   const float* sbet = sb + 768;
@@ -143,145 +153,157 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, const float (
     }
   }
   const bool ln_gate = lna && p.ln_cols == 1;
-  // on-the-fly LayerNorm of the residual rows / partial output statistics: rows it*8 + sub of the transposed layout
-  float r_mean[2], r_rstd[2], st1[2][2], st2[2][2];
+  // on-the-fly LayerNorm of the residual rows / running output statistics of the current half: rows 4*it + rq
+  float r_mean[4], r_rstd[4], st1[4], st2[4];
 #pragma unroll
-  for (int it = 0; it < 2; ++it) {
+  for (int it = 0; it < 4; ++it) {
     r_mean[it] = 0.f; r_rstd[it] = 1.f;
-    st1[0][it] = st1[1][it] = st2[0][it] = st2[1][it] = 0.f;
+    st1[it] = st2[it] = 0.f;
     if (lnr) {
-      const int row = row_base + it * 8 + sub;
+      const int row = row_base + it * 4 + rq;
       if (row < p.M) {
         const float2 ms = __ldg(reinterpret_cast<const float2*>(p.res_stats) + row);
         r_mean[it] = ms.x; r_rstd[it] = ms.y;
       }
     }
   }
-  auto load_mr = [&](int j, float4 (&mm_)[2], float4 (&rr_)[2]) {
-    const int col = tn * bn_out + j + kc * 4;
-    const bool col_ok = col < n_out;
+  // fold the (sum, sum of squares) of statistics half hf over the row's four column groups and let lane c8 == 0 write them
+  auto flush_stats = [&](int hf) {
 #pragma unroll
-    for (int it = 0; it < 2; ++it) {
-      const int row = row_base + it * 8 + sub;
+    for (int it = 0; it < 4; ++it) {
+      float s1 = st1[it], s2 = st2[it];
+      s1 += __shfl_xor_sync(0xffffffffu, s1, 1); s2 += __shfl_xor_sync(0xffffffffu, s2, 1);
+      s1 += __shfl_xor_sync(0xffffffffu, s1, 2); s2 += __shfl_xor_sync(0xffffffffu, s2, 2);
+      const int row = row_base + it * 4 + rq;
+      if (c8 == 0 && row < p.M) reinterpret_cast<float2*>(p.stats_out)[(size_t)row * p.stats_parts + tn * 2 + hf] = make_float2(s1, s2);
+      st1[it] = st2[it] = 0.f;
+    }
+  };
+  auto load_mr = [&](int j, float4 (&mm_)[4], float4 (&rr_)[4]) {
+    const int col = tn * bn_out + j + c8 * 4;
+    const bool col_ok = j < bn_out && col < n_out;
+#pragma unroll
+    for (int it = 0; it < 4; ++it) {
+      const int row = row_base + it * 4 + rq;
       const bool ok = col_ok && row < p.M;
       if (has_mul) mm_[it] = ok ? __ldg(reinterpret_cast<const float4*>(p.mul + (size_t)row * p.ld_mul + col)) : make_float4(1.f, 1.f, 1.f, 1.f);
       if (has_res) rr_[it] = ok ? __ldg(reinterpret_cast<const float4*>(p.residual + (size_t)row * p.ld_res + col)) : make_float4(0.f, 0.f, 0.f, 0.f);
     }
   };
-  // The multiplier / residual rows of sub-chunk s+1 are requested before sub-chunk s is processed (one sub-chunk of register
-  // prefetch), so their latency overlaps the arithmetic, the transpose and the stores of the sub-chunk in hand.
-  float4 mm[2], rr[2], mm_n[2], rr_n[2];
-  load_mr(0, mm, rr);
-  const int wsw = (sub >> 1) & 3;  // transpose swizzle of this thread's fragment rows (sub and sub + 8 share it)
+  auto chunk_of = [](int k) { return k < NEV ? 2 * k : 2 * (k - NEV) + 1; };  // processing order: even chunks, then odd ones
+  float4 mm[NB][4], rr[NB][4];
+  const int wsw = (sub & 3) << 1;  // transpose swizzle of this thread's fragment rows (sub and sub + 8 share it)
+  const int rsw = rq << 1;         // and of its transposed rows 4*it + rq
 #pragma unroll
-  for (int s = 0; s < BN / 16; ++s) {
-    const int j = s * 16;
+  for (int k = 0; k < NCH; ++k) {
+    const int c = chunk_of(k);
+    const int j = c * 32;
+    if (k % NB == 0) {
+#pragma unroll
+      for (int b = 0; b < NB; ++b)
+        if (k + b < NCH) load_mr(chunk_of(k + b) * 32, mm[b], rr[b]);
+    }
     if (j < bn_out) {
-      const int col = tn * bn_out + j + kc * 4;
-      const bool col_ok = col < n_out;  // n_out % 4 == 0 (checked on the host)
-      if (j + 16 < bn_out) load_mr(j + 16, mm_n, rr_n);
-      float v[8], g[8], x[8];
 #pragma unroll
-      for (int i = 0; i < 8; ++i) v[i] = acc[s * 8 + i];
-      if (glu) acc_group16<BN>(acc, s + bn_out / 16, g);
-      // fragment element i: row sub + 8*((i>>1)&1), column j + 8*(i>>2) + 2*kc + (i&1)
+      for (int u = 0; u < 2; ++u) {  // the chunk's two 16-column fragment groups
+        const int s = 2 * c + u;
+        float v[8], g[8], x[8];
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int c = j + 8 * (i >> 2) + 2 * kc + (i & 1);
-        const int h = (i >> 1) & 1;
-        float a;
-        if (lna) a = fmaf(fmaf(-a_mean[h], sc1[c], v[i] * scale), a_rstd[h], sb[c]);
-        else a = fmaf(v[i], scale, sb[c]);
-        if (glu) {
-          float gt;
-          if (ln_gate) gt = fmaf(fmaf(-a_mean[h], sc1[bn_out + c], g[i] * scale), a_rstd[h], sb[bn_out + c]);
-          else gt = fmaf(g[i], scale, sb[bn_out + c]);
-          a = E::GENERIC ? apply_act(p.act, a) : act_ct<E::ACT>(a);
-          x[i] = a * gt;
-        } else {
-          x[i] = E::GENERIC ? apply_act(p.act, a) : act_ct<E::ACT>(a);
-        }
-      }
+        for (int i = 0; i < 8; ++i) v[i] = acc[s * 8 + i];
+        if (glu) acc_group16<BN>(acc, s + bn_out / 16, g);
+        // fragment element i: row sub + 8*((i>>1)&1), column 16s + 8*(i>>2) + 2*kc + (i&1)
 #pragma unroll
-      for (int q = 0; q < 2; ++q)     // column group 8q .. 8q+7: 16-byte chunk 2q + kc/2, float2 at (2*kc) % 4
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int r = sub + 8 * h;
-          const int ch = (2 * q + (kc >> 1)) ^ wsw;
-          *reinterpret_cast<float2*>(st + r * 16 + ch * 4 + (2 * kc & 3)) = make_float2(x[4 * q + 2 * h], x[4 * q + 2 * h + 1]);
-        }
-      __syncwarp();
-      float4 y[2];
-#pragma unroll
-      for (int it = 0; it < 2; ++it) {
-        const int r = it * 8 + sub;
-        y[it] = *reinterpret_cast<const float4*>(st + r * 16 + ((kc ^ ((r >> 1) & 3)) << 2));
-      }
-      const int half = (j >> 5) & 1;
-#pragma unroll
-      for (int it = 0; it < 2; ++it) {
-        const int row = row_base + it * 8 + sub;
-        if (!(col_ok && row < p.M)) continue;
-        float4 o = y[it];
-        if (has_mul) { o.x *= mm[it].x; o.y *= mm[it].y; o.z *= mm[it].z; o.w *= mm[it].w; }
-        if (has_res) {
-          float4 r = rr[it];
-          if (lnr) {
-            const float4 gm = *reinterpret_cast<const float4*>(sgam + j + kc * 4);
-            const float4 bt = *reinterpret_cast<const float4*>(sbet + j + kc * 4);
-            const float m_ = r_mean[it], s_ = r_rstd[it];
-            r.x = fmaf((r.x - m_) * s_, gm.x, bt.x); r.y = fmaf((r.y - m_) * s_, gm.y, bt.y);
-            r.z = fmaf((r.z - m_) * s_, gm.z, bt.z); r.w = fmaf((r.w - m_) * s_, gm.w, bt.w);
+        for (int i = 0; i < 8; ++i) {
+          const int cc = s * 16 + 8 * (i >> 2) + 2 * kc + (i & 1);
+          const int h = (i >> 1) & 1;
+          float a;
+          if (lna) a = fmaf(fmaf(-a_mean[h], sc1[cc], v[i] * scale), a_rstd[h], sb[cc]);
+          else a = fmaf(v[i], scale, sb[cc]);
+          if (glu) {
+            float gt;
+            if (ln_gate) gt = fmaf(fmaf(-a_mean[h], sc1[bn_out + cc], g[i] * scale), a_rstd[h], sb[bn_out + cc]);
+            else gt = fmaf(g[i], scale, sb[bn_out + cc]);
+            a = E::GENERIC ? apply_act(p.act, a) : act_ct<E::ACT>(a);
+            x[i] = a * gt;
+          } else {
+            x[i] = E::GENERIC ? apply_act(p.act, a) : act_ct<E::ACT>(a);
           }
-          o.x += r.x; o.y += r.y; o.z += r.z; o.w += r.w;
+        }
+#pragma unroll
+        for (int q = 0; q < 2; ++q)     // chunk columns 16u + 8q .. +7: 16-byte chunk 4u + 2q + kc/2, float2 at (2*kc) % 4
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int r = sub + 8 * h;
+            const int ch = (4 * u + 2 * q + (kc >> 1)) ^ wsw;
+            *reinterpret_cast<float2*>(st + r * 32 + ch * 4 + (2 * kc & 3)) = make_float2(x[4 * q + 2 * h], x[4 * q + 2 * h + 1]);
+          }
+      }
+      __syncwarp();
+      float4 y[4];
+#pragma unroll
+      for (int it = 0; it < 4; ++it) y[it] = *reinterpret_cast<const float4*>(st + (it * 4 + rq) * 32 + ((c8 ^ rsw) << 2));
+      const int col = tn * bn_out + j + c8 * 4;
+      const bool col_ok = col < n_out;  // n_out % 4 == 0 (checked on the host)
+      float4 gm, bt;
+      if (lnr) {
+        gm = *reinterpret_cast<const float4*>(sgam + j + c8 * 4);
+        bt = *reinterpret_cast<const float4*>(sbet + j + c8 * 4);
+      }
+#pragma unroll
+      for (int it = 0; it < 4; ++it) {
+        const int row = row_base + it * 4 + rq;
+        float q1 = 0.f, q2 = 0.f;
+        if (col_ok && row < p.M) {
+          float4 o = y[it];
+          if (has_mul) { const float4 m = mm[k % NB][it]; o.x *= m.x; o.y *= m.y; o.z *= m.z; o.w *= m.w; }
+          if (has_res) {
+            float4 r = rr[k % NB][it];
+            if (lnr) {
+              const float m_ = r_mean[it], s_ = r_rstd[it];
+              r.x = fmaf((r.x - m_) * s_, gm.x, bt.x); r.y = fmaf((r.y - m_) * s_, gm.y, bt.y);
+              r.z = fmaf((r.z - m_) * s_, gm.z, bt.z); r.w = fmaf((r.w - m_) * s_, gm.w, bt.w);
+            }
+            o.x += r.x; o.y += r.y; o.z += r.z; o.w += r.w;
+          }
+          if (stats) {
+            q1 = (o.x + o.y) + (o.z + o.w);
+            q2 = fmaf(o.x, o.x, o.y * o.y) + fmaf(o.z, o.z, o.w * o.w);
+          }
+          if (o32) *reinterpret_cast<float4*>(p.out_f32 + (size_t)row * p.ld_o32 + col) = o;
+          if (o16) {
+            if (p.out_lo8) {  // fp16 hi + e4m3 cross-term views for an "f16f8" consumer
+              uint2 h16;
+              uint32_t l8, h8;
+              split4_f8(o, F8_ACT_LO_SCALE, F8_ACT_HI_SCALE, h16, l8, h8);
+              *reinterpret_cast<uint2*>(p.out_hi + (size_t)row * p.ld_o16 + col) = h16;
+              *reinterpret_cast<uint32_t*>(p.out_lo8 + (size_t)row * p.ld_o8 + col) = l8;
+              *reinterpret_cast<uint32_t*>(p.out_hi8 + (size_t)row * p.ld_o8 + col) = h8;
+            } else {
+              uint2 hi, lo;
+              if (E::GENERIC) {
+                if (p.dtype == DT_F16) split4<DT_F16>(o, hi, lo); else split4<DT_BF16>(o, hi, lo);
+              } else {
+                split4<E::DT>(o, hi, lo);
+              }
+              *reinterpret_cast<uint2*>(p.out_hi + (size_t)row * p.ld_o16 + col) = hi;
+              if (p.out_lo) *reinterpret_cast<uint2*>(p.out_lo + (size_t)row * p.ld_o16 + col) = lo;
+            }
+          }
         }
         if (stats) {
-          st1[half][it] += (o.x + o.y) + (o.z + o.w);
-          st2[half][it] += fmaf(o.x, o.x, o.y * o.y) + fmaf(o.z, o.z, o.w * o.w);
-        }
-        if (o32) *reinterpret_cast<float4*>(p.out_f32 + (size_t)row * p.ld_o32 + col) = o;
-        if (o16) {
-          if (p.out_lo8) {  // fp16 hi + e4m3 cross-term views for an "f16f8" consumer
-            uint2 h16;
-            uint32_t l8, h8;
-            split4_f8(o, F8_ACT_LO_SCALE, F8_ACT_HI_SCALE, h16, l8, h8);
-            *reinterpret_cast<uint2*>(p.out_hi + (size_t)row * p.ld_o16 + col) = h16;
-            *reinterpret_cast<uint32_t*>(p.out_lo8 + (size_t)row * p.ld_o8 + col) = l8;
-            *reinterpret_cast<uint32_t*>(p.out_hi8 + (size_t)row * p.ld_o8 + col) = h8;
-          } else {
-            uint2 hi, lo;
-            if (E::GENERIC) {
-              if (p.dtype == DT_F16) split4<DT_F16>(o, hi, lo); else split4<DT_BF16>(o, hi, lo);
-            } else {
-              split4<E::DT>(o, hi, lo);
-            }
-            *reinterpret_cast<uint2*>(p.out_hi + (size_t)row * p.ld_o16 + col) = hi;
-            if (p.out_lo) *reinterpret_cast<uint2*>(p.out_lo + (size_t)row * p.ld_o16 + col) = lo;
-          }
+          // lanes c8 and c8 ^ 4 hold the two 16-column sub-chunks of this 4-column group; both add them in sub-chunk order.  A
+          // column past n_out adds +0, which leaves the sum unchanged (it starts at +0 and so is never -0)
+          const float p1 = __shfl_xor_sync(0xffffffffu, q1, 4), p2 = __shfl_xor_sync(0xffffffffu, q2, 4);
+          const bool first = c8 < 4;
+          st1[it] = (st1[it] + (first ? q1 : p1)) + (first ? p1 : q1);
+          st2[it] = (st2[it] + (first ? q2 : p2)) + (first ? p2 : q2);
         }
       }
       __syncwarp();
-#pragma unroll
-      for (int it = 0; it < 2; ++it) {
-        if (has_mul) mm[it] = mm_n[it];
-        if (has_res) rr[it] = rr_n[it];
-      }
     }
+    if (stats && k == NEV - 1) flush_stats(0);
   }
-  if (stats) {
-    // every row's 4 column-group lanes hold partial sums over its half of the columns: fold them (fixed order -> run-to-run and
-    // batch-slice deterministic) and let the kc == 0 lane write the (n-tile, half) partials
-#pragma unroll
-    for (int hf = 0; hf < 2; ++hf)
-#pragma unroll
-      for (int it = 0; it < 2; ++it) {
-        float s1 = st1[hf][it], s2 = st2[hf][it];
-        s1 += __shfl_xor_sync(0xffffffffu, s1, 1); s2 += __shfl_xor_sync(0xffffffffu, s2, 1);
-        s1 += __shfl_xor_sync(0xffffffffu, s1, 2); s2 += __shfl_xor_sync(0xffffffffu, s2, 2);
-        const int row = row_base + it * 8 + sub;
-        if (kc == 0 && row < p.M) reinterpret_cast<float2*>(p.stats_out)[(size_t)row * p.stats_parts + tn * 2 + hf] = make_float2(s1, s2);
-      }
-  }
+  if (stats) flush_stats(1);
 }
 
 template <class E, int SPLIT, int BN>
@@ -364,7 +386,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_tc_kernel(const __grid_c
   setmaxnreg_inc<GEMM_CONSUMER_REGS>();
   const int wg = warp >> 2;
   const int et = threadIdx.x;  // 0..255
-  float* st = staging + warp * (16 * 16);
+  float* st = staging + warp * (16 * 32);
   const bool glu = E::GENERIC ? (p.glu != 0) : E::GLU;
   const int n_out = glu ? p.N / 2 : p.N;
   const int bn_out = glu ? BN / 2 : BN;

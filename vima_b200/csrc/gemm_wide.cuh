@@ -144,7 +144,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_wide_kernel(const __grid
   setmaxnreg_inc<GEMM_CONSUMER_REGS>();
   const int wg = warp >> 2;
   const int et = threadIdx.x;  // 0..255
-  float* st = staging + warp * (16 * 16);
+  float* st = staging + warp * (16 * 32);
   const bool glu = E::GENERIC ? (p.glu != 0) : E::GLU;
   const int n_out = glu ? p.N / 2 : p.N;
   const int bn_out = glu ? BN / 2 : BN;
